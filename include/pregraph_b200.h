@@ -141,10 +141,22 @@ size_t pgb200_cut_chunk(const char *buf, size_t n, int fastq);
 
 /* f2 (SURVEY 8f): binary edge sidecar `<prefix>.edge.b200` for a `contig` that links csrc/contig_sidecar.c -- the edges without
  * the gzip'ed text (the reference's loader: loadPreGraph.c:448-544).  Written by the stage when PGB200_EDGE_SIDECAR is set (the
- * byte-identical .edge.gz is still written, unless the value is "only").  This entry point converts edge TEXT (the uncompressed content of an .edge.gz) on the host:
- *   48-byte header { char magic[8] = "PGB2EDGE"; u32 version = 1, K, kmer_words (2 | 4), 0; u64 n_records, num_ed, 0 }
- *   per record    { i32 length, cvg, bal_ed, seq_bytes = length / 4 + 1; u64 from[kmer_words], to[kmer_words]; u8 seq[seq_bytes] }
+ * byte-identical .edge.gz is still written, unless the value is "only").  The file is this header, then n_records records
+ *   { i32 length, cvg, bal_ed, seq_bytes = length / 4 + 1; u64 from[kmer_words], to[kmer_words]; u8 seq[seq_bytes] }
  *   (seq: 4 bases per byte, first base in bits 7:6, codes A0 C1 T2 G3 -- writeChar2tightString, seq.c:81)                         */
+#define PGB200_SIDECAR_MAGIC "PGB2EDGE"   /* the 8 bytes of magic[], no terminating NUL */
+#define PGB200_SIDECAR_VERSION 1
+typedef struct pgb200_edge_sidecar_header {
+    char magic[8];
+    uint32_t version, K, kmer_words, reserved0;   /* kmer_words: 2 (63-mer flavour) or 4 (127-mer flavour); reserved0 = 0 */
+    uint64_t n_records, num_ed, reserved1;        /* num_ed: edges including twins (the EDGEs line of .preGraphBasic)     */
+} pgb200_edge_sidecar_header;
+#ifdef __cplusplus
+static_assert(sizeof(pgb200_edge_sidecar_header) == 48, "the sidecar header is 48 bytes");
+#else
+_Static_assert(sizeof(pgb200_edge_sidecar_header) == 48, "the sidecar header is 48 bytes");
+#endif
+/* Converts edge TEXT (the uncompressed content of an .edge.gz) into a sidecar, on the host. */
 int pgb200_edge_text_to_sidecar(const char *text, size_t nbytes, int K, int flavour127, uint64_t num_ed, const char *path);
 /* The way back, host only: `<prefix>.edge.b200` -> the byte-identical `<prefix>.edge.gz` (record text of output_pregraph.c:88-110, deflated
  * like the stage does).  For pipelines that ran the stage with PGB200_EDGE_SIDECAR=only and want the .edge.gz later / in the background. */

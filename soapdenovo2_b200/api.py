@@ -220,7 +220,7 @@ def plan_files(cfg: str):
     lib = load()
     buf = C.create_string_buffer(1 << 20)
     if lib.pgb200_plan_files(cfg.encode(), buf, len(buf)):
-        raise EngineError("plan too large")
+        raise EngineError(lib.pgb200_last_error().decode())
     lines = buf.value.decode().splitlines()
     plan = []
     for l in lines[1:]:

@@ -1,16 +1,12 @@
 /* contig_sidecar.c -- f2 (SURVEY 8f): the `contig` side of the pregraph -> contig hand-over, without the gzip'ed text.
  *
  * The engine can write the edges it builds as a binary sidecar `<prefix>.edge.b200` next to the byte-identical `.edge.gz`
- * (PGB200_EDGE_SIDECAR=1; format below and in include/pregraph_b200.h).  This file is the reader a maintainer adds to SOAPdenovo2:
+ * (PGB200_EDGE_SIDECAR=1; format: pgb200_edge_sidecar_header in include/pregraph_b200.h).  This file is the reader a maintainer adds to SOAPdenovo2:
  * a `loadEdge()` that fills `edge_array` from the sidecar exactly as the reference's text loader does (loadPreGraph.c:448-544:
  * same allocation, same fields, same buildReverseComplementEdge / createArcMemo / loadPreArcs calls) and falls back to that loader
  * when there is no sidecar.  Nothing of the reference is modified in source: scripts/link_dropin.sh renames the original symbol in
  * the reference's OWN object (`objcopy --redefine-sym loadEdge=loadEdge_text loadPreGraph.o`) and links this file beside it.
  * It is compiled against the reference's headers where they lie (-I$REF/standardPregraph/inc, -DMER63 | -DMER127).
- *
- * Sidecar: 48-byte header { char magic[8] = "PGB2EDGE"; u32 version = 1; u32 K; u32 kmer_words (2 | 4); u32 reserved; u64 n_records;
- * u64 num_ed; u64 reserved }, then per record { i32 length; i32 cvg; i32 bal_ed; u32 seq_bytes = length / 4 + 1;
- * u64 from[kmer_words]; u64 to[kmer_words]; u8 seq[seq_bytes] (4 bases per byte, first base in bits 7:6: writeChar2tightString) }.
  */
 #include <stdio.h>
 #include <stdlib.h>
@@ -20,6 +16,7 @@
 #include "kmerhash.h"
 #include "extfunc.h"
 #include "extvab.h"
+#include "../../include/pregraph_b200.h"
 
 extern void loadEdge_text(char *graphfile);                 /* the reference's loadEdge, renamed at link time */
 extern void buildReverseComplementEdge(unsigned int edgeno);  /* static in loadPreGraph.c; made global in the object at link time */
@@ -83,24 +80,18 @@ static void sidecar_load_prearcs(char *graphfile)
     fclose(fp);
 }
 
-typedef struct {
-    char magic[8];
-    unsigned int version, K, kmer_words, reserved0;
-    unsigned long long n_records, num_ed, reserved1;
-} SidecarHeader;
-
 void loadEdge(char *graphfile)
 {
     char name[512];
     FILE *fp;
-    SidecarHeader h;
+    pgb200_edge_sidecar_header h;
     unsigned long long r;
     int index = -1;
     unsigned int j;
     snprintf(name, sizeof name, "%s.edge.b200", graphfile);
     fp = fopen(name, "rb");
     if (!fp) { loadEdge_text(graphfile); return; }
-    if (fread(&h, sizeof h, 1, fp) != 1 || memcmp(h.magic, "PGB2EDGE", 8) != 0 || h.version != 1 || h.kmer_words != sizeof(Kmer) / 8) {
+    if (fread(&h, sizeof h, 1, fp) != 1 || memcmp(h.magic, PGB200_SIDECAR_MAGIC, 8) != 0 || h.version != PGB200_SIDECAR_VERSION || h.kmer_words != sizeof(Kmer) / 8) {
         fprintf(stderr, "%s is not an edge sidecar of this build; reading %s.edge.gz instead.\n", name, graphfile);
         fclose(fp);
         loadEdge_text(graphfile);

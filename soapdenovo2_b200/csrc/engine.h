@@ -3,10 +3,14 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <ctime>
 #include <string>
 #include <vector>
 
 namespace pgb {
+
+// monotonic host clock in milliseconds
+inline double host_now() { struct timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e3 + t.tv_nsec * 1e-6; }
 
 struct PgParams {
     int K = 23;              // overlaplen after the reference's fix-ups (pregraph.c:71-97)

@@ -60,7 +60,6 @@ using Stream = CudaOwned<cudaStream_t, cudaStreamDestroy>;
 using Event = CudaOwned<cudaEvent_t, cudaEventDestroy>;
 template <class T> using Pinned = CudaOwned<T*, free_pinned<T>>;
 
-inline double host_now() { struct timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e3 + t.tv_nsec * 1e-6; }
 inline u64 next_pow2(u64 x) { u64 p = 1; while (p < x) p <<= 1; return p; }
 
 // One fed text chunk, decoded: 2-bit packed reads (LSB-first, W64 words per read) + lengths.  Stays resident in HBM so

@@ -72,6 +72,29 @@ def test_malformed_records_are_rejected(text, fastq):
     eng.close()
 
 
+def test_graph_phases_through_the_c_abi(tmp_path, monkeypatch):
+    """pgb200_remove_tips / kmer2edges / read2edge / output_vertex write what the stage writes, and the edge sidecar that
+    kmer2edges writes carries the edge count of the edges it just built."""
+    import struct
+    cfg = synth.scenario_se_fasta(str(tmp_path))
+    ref, pre = str(tmp_path / "ref"), str(tmp_path / "abi")
+    _oracle(0, cfg, ref, 31, 3, ("-a", "1", "-R"))
+    mrl, plan = api.plan_files(cfg)
+    eng = api.PregraphEngine(K=31, P=3, initG=1, repsTie=1, max_rd_len=mrl)
+    n = 0
+    for mate, fq, rev, cut, path in plan:
+        assert mate == -1
+        n += eng.feed_text(open(path, "rb").read(), fastq=bool(fq), ord_base=n, reverse_seq=rev, maxlen=cut)
+    eng.finish_pass1(); eng.sweeps(); eng.build_layout()
+    monkeypatch.setenv("PGB200_EDGE_SIDECAR", "1")
+    eng.remove_tips(); eng.kmer2edges(pre); eng.read2edge(pre); eng.output_vertex(pre)
+    util.compare(ref, pre, util.SUFFIXES_R[1:])   # everything but the .kmerFreq, which only the stage writes
+    magic, version, K, kw, _, n_rec, num_ed, _ = struct.unpack("<8sIIIIQQQ", open(pre + ".edge.b200", "rb").read(48))
+    assert (magic, version, K, kw) == (b"PGB2EDGE", 1, 31, 2)
+    assert num_ed == eng.graph.num_ed > 0 and n_rec == eng.graph.edges
+    eng.close()
+
+
 def test_truncation_and_reverse_via_api(tmp_path):
     """maxlen truncation and reverse_seq give the same table as feeding the pre-truncated / pre-reversed reads."""
     import numpy as np

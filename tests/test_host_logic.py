@@ -1,6 +1,7 @@
 """CPU: the host-side read-stream plan (config parsing, library sort, file-type order, truncation) against the ORDER in which the
 unmodified reference binary opens the files (its "Import reads from file:" stderr lines)."""
 import os
+import re
 import subprocess
 
 import pytest
@@ -100,3 +101,49 @@ def test_chunk_cut_fasta():
     rec = len(fa) // 4
     assert api.cut_chunk(fa[: 3 * rec + 4], False) == 3 * rec      # '>' starts a record, the rest of it follows with the next read
     assert api.cut_chunk(fa[: rec - 2], False) == 0
+
+
+_STAGE_HEAD = "\n********************\nPregraph\n********************\n\nParameters: pregraph -s {cfg} -o {out} \n\n"
+
+
+def _stage(tmp_path, cfg_text):
+    """The CLI on one config (None: the file does not exist): exit status, stderr and the argument paths."""
+    cfg, out = str(tmp_path / "lib.cfg"), str(tmp_path / "out")
+    if cfg_text is not None:
+        open(cfg, "w").write(cfg_text)
+    r = subprocess.run([api.BIN63, "pregraph", "-s", cfg, "-o", out], capture_output=True, text=True)
+    return r.returncode, r.stderr, cfg, out
+
+
+@pytest.mark.parametrize("cfg_text,message", [
+    (None, "Cannot open {cfg}. Now exit to system..."),
+    ("max_rd_len=100\n", "Config file error: no [LIB] in file"),
+    ("[LIB]\navg_ins=200\nf1=/x/a.fa\n", 'Config file error: the number of mark "f1" is not the same as "f2"!'),
+    ("[LIB]\nb=/x/a.bam\n", "pgb200: BAM input (b=) is not supported by the GPU engine"),
+    ("[LIB]\nf1=/x/a.fa\nf2=/x/b.fa\n", "Config file error: PE reads need avg_ins in [LIB] 1"),
+])
+def test_cli_config_errors(tmp_path, cfg_text, message):
+    """A bad config ends the stage with status 255 (exit(-1), as the reference) after the lines it printed so far."""
+    rc, err, cfg, out = _stage(tmp_path, cfg_text)
+    assert rc == 255
+    assert err == _STAGE_HEAD.format(cfg=cfg, out=out) + message.format(cfg=cfg) + "\n"
+
+
+def test_cli_without_gpu_fails_at_engine_creation(tmp_path):
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("GPU present")
+    rc, err, cfg, out = _stage(tmp_path, "[LIB]\nf=/x/a.fa\n")
+    head = _STAGE_HEAD.format(cfg=cfg, out=out) + f"In {cfg}, 1 lib(s), maximum read length 100, maximum name length 256.\n\n"
+    assert rc == 255 and err.startswith(head)
+    assert re.fullmatch(r"pgb200: CUDA error \w+ at \w+\.cu:\d+: [^\n]+\n", err[len(head):]), err
+
+
+def test_plan_files_reports_a_bad_config_as_an_error(tmp_path):
+    """The host-logic entry point returns an error with the stage's message; it does not end the calling process."""
+    cfg = str(tmp_path / "absent.cfg")
+    with pytest.raises(api.EngineError, match=re.escape(f"Cannot open {cfg}. Now exit to system...")):
+        api.plan_files(cfg)
+    open(cfg, "w").write("max_rd_len=100\n")
+    with pytest.raises(api.EngineError, match=re.escape("Config file error: no [LIB] in file")):
+        api.plan_files(cfg)
