@@ -14,6 +14,12 @@
  *                                 reference's -DMER63 / -DMER127 (Makefile:51-66) and keeps the `all` pipeline's globals.
  *   pgb200_pregraph_main          the stage with the flavour as an argument (what the shim and the CLI front ends call).
  *                                 PGB200_GPUS=n shards pass 1 over n GPUs of the box (see pgb200_xchg_* below).
+ *   pgb200_map_main               int call_align(int argc, char **argv)                map.c:96.  The `map` stage: same argv contract
+ *                                 ("map -s cfg -g prefix [-f] [-p n -k k -h len]"), same .readOnContig.gz / .readInGap.gz / .peGrads
+ *                                 (and with -f .shortreadInGap.gz / .PEreadOnContig.gz), same stderr counters; -p is a layout
+ *                                 parameter of .readInGap.gz, as in the reference.  One GPU (PGB200_DEVICE).  Long-read
+ *                                 libraries (asm_flags=4) and BAM are refused.  Returns 0; a failure ends the process, as there.
+ *                                 The drop-in's call_align (csrc/pregraph_shim.c) calls it.
  *   pgb200_feed_text + pgb200_finish_pass1 + pgb200_sweeps
  *                                 boolean prlRead2HashTable(char *libfile, char *outfile)   prlHashReads.c:304
  *                                 (readers readseq1by1.c:138-360, chopKmer4read :163-259, put_kmerset newhash.c:473-528,
@@ -164,6 +170,7 @@ int pgb200_sidecar_to_edge_gz(const char *prefix);
 
 /* The drop-in stage entry points. */
 int pgb200_pregraph_main(int argc, char **argv, int flavour127);
+int pgb200_map_main(int argc, char **argv, int flavour127);
 int call_pregraph(int argc, char **argv);
 
 #ifdef __cplusplus

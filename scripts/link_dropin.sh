@@ -1,8 +1,10 @@
 #!/bin/bash
 # Link-level drop-in check (INTEGRATION.md section 1): the reference's OWN objects (oracle/_ref/o{63,127}/*.o, compiled unmodified
 # from /root/reference by oracle/Makefile) minus the six files the engine replaces, plus pregraph_shim.o and libpregraph_b200.so.
-# The result, oracle/_ref/SOAPdenovo-{63,127}mer-b200, is the reference's main() / contig / map / scaff around the GPU pregraph:
-#   SOAPdenovo-63mer-b200 pregraph ... | contig ... | all ...      (tests/test_gpu_dropin.py compares it with the unmodified binary)
+# The result, oracle/_ref/SOAPdenovo-{63,127}mer-b200, is the reference's main() / contig / scaff around the GPU pregraph and the
+# GPU map (map.o, prlHashCtg.o and prlRead2Ctg.o are left out: nothing else uses their symbols; the shim's call_align replaces them):
+#   SOAPdenovo-63mer-b200 pregraph ... | contig ... | map ... | all ...   (tests/test_gpu_dropin.py, tests/test_gpu_map_dropin.py compare
+#   them with the unmodified binary)
 # f2: the same binaries read the engine's binary edge sidecar (<prefix>.edge.b200) when there is one -- csrc/contig_sidecar.c is linked
 # beside the reference's loadPreGraph.o, whose loadEdge symbol is renamed (and whose static buildReverseComplementEdge is made global)
 # IN THE OBJECT with objcopy; no reference source is touched or copied.
@@ -18,7 +20,7 @@ fi
 for fl in 63 127; do
   [ -d $REF/o$fl ] || { echo "link_dropin: $REF/o$fl missing (run make -C oracle ref where /root/reference exists)"; exit 2; }
   T=$REF/o$fl/.b200_tmp; rm -rf $T; mkdir -p $T
-  objs=$(ls $REF/o$fl/*.o | grep -v -E '/(pregraph|prlHashReads|cutTipPreGraph|node2edge|prlRead2path|output_pregraph|loadPreGraph)\.o$')
+  objs=$(ls $REF/o$fl/*.o | grep -v -E '/(pregraph|prlHashReads|cutTipPreGraph|node2edge|prlRead2path|output_pregraph|loadPreGraph|map|prlHashCtg|prlRead2Ctg)\.o$')
   gcc -O2 -c -DPGB_FLAVOUR127=$([ $fl = 127 ] && echo 1 || echo 0) soapdenovo2_b200/csrc/pregraph_shim.c -o $T/pregraph_shim.o
   objcopy --redefine-sym loadEdge=loadEdge_text --globalize-symbol=buildReverseComplementEdge $REF/o$fl/loadPreGraph.o $T/loadPreGraph_renamed.o
   gcc -O2 -w -fcommon -c -DMER$fl -I$REFSRC/standardPregraph/inc soapdenovo2_b200/csrc/contig_sidecar.c -o $T/contig_sidecar.o

@@ -22,7 +22,7 @@ EXPORTS = [
     "pgb200_xchg_setup", "pgb200_xchg_export", "pgb200_xchg_import", "pgb200_xchg_base", "pgb200_xchg_import_ptr", "pgb200_xchg_fence", "pgb200_flush", "pgb200_xchg_room", "pgb200_absorb",
     "pgb200_finish_pass1", "pgb200_reset_pass1", "pgb200_sweeps",
     "pgb200_build_layout", "pgb200_node_count", "pgb200_dump_nodes", "pgb200_sample_table", "pgb200_remove_tips", "pgb200_kmer2edges",
-    "pgb200_read2edge", "pgb200_output_vertex", "pgb200_edge_text_to_sidecar", "pgb200_sidecar_to_edge_gz", "pgb200_plan_files", "pgb200_cut_chunk", "pgb200_pregraph_main", "call_pregraph",
+    "pgb200_read2edge", "pgb200_output_vertex", "pgb200_edge_text_to_sidecar", "pgb200_sidecar_to_edge_gz", "pgb200_plan_files", "pgb200_cut_chunk", "pgb200_pregraph_main", "pgb200_map_main", "call_pregraph",
 ]
 
 
@@ -91,6 +91,7 @@ def load():
     lib.pgb200_cut_chunk.restype = C.c_size_t
     lib.pgb200_cut_chunk.argtypes = [C.c_char_p, C.c_size_t, C.c_int]
     lib.pgb200_pregraph_main.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.c_int]
+    lib.pgb200_map_main.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.c_int]
     _lib = lib
     return lib
 

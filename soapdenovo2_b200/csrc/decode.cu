@@ -283,13 +283,70 @@ __global__ void __launch_bounds__(256) k_decode_fix(const unsigned char* __restr
     if (threadIdx.x == 0 && (s_inst | s_kept)) { atomicAdd(&counters[C_INSTANCES], s_inst); atomicAdd(&counters[C_KEPT], s_kept); }
 }
 
-// ------------------------------------------------------------------------------------------------ feed_text
-template <int NW>
-void EngineT<NW>::check_format_counter() {
-    if (h_cnt_[C_BADFMT])
+// ------------------------------------------------------------------------------------------------ the decode of one text chunk
+void check_format(const u64* h_cnt) {
+    if (h_cnt[C_BADFMT])
         throw std::runtime_error("pgb200: input is not single-line FASTA / 4-line FASTQ (a header line does not start with '>' / '@', or a FASTQ "
                                  "separator line does not start with '+'); multi-line FASTA is not supported");
 }
+
+DecodeLines decode_lines(const unsigned char* d_text, size_t nbytes, int fastq, int n_sm, DevBuf& scan_buf, DevBuf& line_buf, u64* d_cnt, u64* h_cnt,
+                         cudaStream_t sd) {
+    const int lshift = fastq ? 2 : 1, lpr = 1 << lshift;
+    const u64 n_tiles = (nbytes + NL_TILE - 1) / NL_TILE;
+    scan_buf.ensure((2 * n_tiles + 16) * sizeof(u32) + scan_scratch_elems(n_tiles) * sizeof(u64) + 256);
+    u32* tile_cnt = scan_buf.template as<u32>();
+    u32* tile_base = tile_cnt + n_tiles + 8;
+    u64* scan_tmp = reinterpret_cast<u64*>((reinterpret_cast<uintptr_t>(tile_base + n_tiles + 8) + 255) & ~(uintptr_t)255);
+    const uint4* t16 = reinterpret_cast<const uint4*>(d_text);
+    const unsigned nl_blocks = (unsigned)std::min<u64>((n_tiles + 7) / 8, (u64)n_sm * 16);
+    k_nl_count<<<nl_blocks, 256, 0, sd>>>(t16, (u64)nbytes, n_tiles, tile_cnt);
+    PG_CUDA(cudaGetLastError());
+    device_scan(TileCntIn{tile_cnt}, TileBaseOut{tile_base}, n_tiles, scan_tmp, d_cnt + C_MISC0, sd);
+    unsigned char* h_last = reinterpret_cast<unsigned char*>(h_cnt + C_COUNT);
+    PG_CUDA(cudaMemcpyAsync(h_last, d_text + nbytes - 1, 1, cudaMemcpyDeviceToHost, sd));
+    PG_CUDA(cudaMemcpyAsync(h_cnt, d_cnt, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, sd));
+    PG_CUDA(cudaStreamSynchronize(sd));
+    check_format(h_cnt);
+    const u64 n_lines = h_cnt[C_MISC0];
+    // a final line without '\n' still counts (the reference's FASTQ path tolerates it; its FASTA path does not)
+    const bool open_tail = *h_last != '\n';
+    DecodeLines L{nullptr, nullptr, nullptr, (n_lines + (open_tail ? 1 : 0)) / lpr};
+    if ((n_lines + (open_tail ? 1 : 0)) % lpr != 0)
+        throw std::runtime_error("pgb200: text chunk does not hold whole FASTA/FASTQ records (line count not a multiple of 2/4)");
+    const u64 n_rec = L.n_rec;
+    if (n_rec == 0) return L;
+    line_buf.ensure(2 * n_rec * sizeof(u32) + n_rec + 256);
+    L.seq_start = line_buf.template as<u32>();
+    L.seq_end = L.seq_start + n_rec;
+    L.bad = reinterpret_cast<u8*>(L.seq_end + n_rec);
+    PG_CUDA(cudaMemsetAsync(L.bad, 0, n_rec, sd));
+    if (open_tail) PG_CUDA(cudaMemsetAsync(L.seq_end, 0, n_rec * sizeof(u32), sd));   // FASTQ: the open line is the quality line
+    k_line_index<<<nl_blocks, 256, 0, sd>>>(t16, (u64)nbytes, n_tiles, tile_base, lshift, n_rec, L.seq_start, L.seq_end, d_cnt);
+    PG_CUDA(cudaGetLastError());
+    if (open_tail && !fastq) {
+        const u32 e = (u32)nbytes;
+        PG_CUDA(cudaMemcpyAsync(L.seq_end + n_rec - 1, &e, sizeof e, cudaMemcpyHostToDevice, sd));
+        PG_CUDA(cudaStreamSynchronize(sd));
+    }
+    return L;
+}
+
+void decode_records(const unsigned char* d_text, size_t nbytes, const DecodeLines& L, int maxlen, int reverse, int K, int W64, int n_sm, u64* words,
+                    u32* lens, u64* d_cnt, cudaStream_t sd) {
+    const u64 n_rec = L.n_rec, total = n_rec * (u64)W64;
+    k_decode_fast<<<(unsigned)std::min<u64>((total + 255) / 256, (u64)n_sm * 64), 256, 0, sd>>>(d_text, (u64)nbytes, L.seq_start, L.seq_end, n_rec, maxlen, W64,
+                                                                                            words, lens, L.bad);
+    PG_CUDA(cudaGetLastError());
+    const u64 fix_warps = (n_rec + 31) / 32;
+    k_decode_fix<<<(unsigned)std::min<u64>((fix_warps + 7) / 8, (u64)n_sm * 32), 256, 0, sd>>>(d_text, L.seq_start, L.seq_end, n_rec, maxlen, reverse, K, W64,
+                                                                                         words, lens, L.bad, d_cnt);
+    PG_CUDA(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------ feed_text
+template <int NW>
+void EngineT<NW>::check_format_counter() { check_format(h_cnt_); }
 
 template <int NW>
 void EngineT<NW>::feed_text(const char* text, size_t nbytes, bool on_device, int fastq, uint64_t ord_base, uint64_t ord_stride,
@@ -331,44 +388,12 @@ void EngineT<NW>::feed_text(const char* text, size_t nbytes, bool on_device, int
         }
     }
     if (maxlen > prm_.max_rd_len) maxlen = prm_.max_rd_len;
-    const int lshift = fastq ? 2 : 1, lpr = 1 << lshift;
-    const u64 n_tiles = (nbytes + NL_TILE - 1) / NL_TILE;
-    scan_buf_.ensure((2 * n_tiles + 16) * sizeof(u32) + scan_scratch_elems(n_tiles) * sizeof(u64) + 256);
-    u32* tile_cnt = scan_buf_.template as<u32>();
-    u32* tile_base = tile_cnt + n_tiles + 8;
-    u64* scan_tmp = reinterpret_cast<u64*>((reinterpret_cast<uintptr_t>(tile_base + n_tiles + 8) + 255) & ~(uintptr_t)255);
-    const uint4* t16 = reinterpret_cast<const uint4*>(d_text);
-    const unsigned nl_blocks = (unsigned)std::min<u64>((n_tiles + 7) / 8, (u64)n_sm_ * 16);
-    k_nl_count<<<nl_blocks, 256, 0, sd>>>(t16, (u64)nbytes, n_tiles, tile_cnt);
-    PG_CUDA(cudaGetLastError());
-    device_scan(TileCntIn{tile_cnt}, TileBaseOut{tile_base}, n_tiles, scan_tmp, d_cnt_ + C_MISC0, sd);
     // ONE host sync per chunk, of the decode stream: line count, last byte, and the counters as they are
-    unsigned char* h_last = reinterpret_cast<unsigned char*>(h_cnt_ + C_COUNT);
-    PG_CUDA(cudaMemcpyAsync(h_last, d_text + nbytes - 1, 1, cudaMemcpyDeviceToHost, sd));
-    read_counters_on(sd);
-    check_format_counter();
-    const u64 n_lines = h_cnt_[C_MISC0];
+    const DecodeLines L = decode_lines(d_text, nbytes, fastq, n_sm_, scan_buf_, line_buf_, d_cnt_, h_cnt_, sd);
+    const u64 n_rec = L.n_rec;
     const u64 have_distinct = h_cnt_[C_DISTINCT];
-    // a final line without '\n' still counts (the reference's FASTQ path tolerates it; its FASTA path does not)
-    const bool open_tail = *h_last != '\n';
-    const u64 n_rec = (n_lines + (open_tail ? 1 : 0)) / lpr;
-    if ((n_lines + (open_tail ? 1 : 0)) % lpr != 0)
-        throw std::runtime_error("pgb200: text chunk does not hold whole FASTA/FASTQ records (line count not a multiple of 2/4)");
     if (n_rec == 0) return;
     t_b = host_now();
-    line_buf_.ensure(2 * n_rec * sizeof(u32) + n_rec + 256);
-    u32* seq_start = line_buf_.template as<u32>();
-    u32* seq_end = seq_start + n_rec;
-    u8* bad = reinterpret_cast<u8*>(seq_end + n_rec);
-    PG_CUDA(cudaMemsetAsync(bad, 0, n_rec, sd));
-    if (open_tail) PG_CUDA(cudaMemsetAsync(seq_end, 0, n_rec * sizeof(u32), sd));   // FASTQ: the open line is the quality line
-    k_line_index<<<nl_blocks, 256, 0, sd>>>(t16, (u64)nbytes, n_tiles, tile_base, lshift, n_rec, seq_start, seq_end, d_cnt_);
-    PG_CUDA(cudaGetLastError());
-    if (open_tail && !fastq) {
-        const u32 e = (u32)nbytes;
-        PG_CUDA(cudaMemcpyAsync(seq_end + n_rec - 1, &e, sizeof e, cudaMemcpyHostToDevice, sd));
-        PG_CUDA(cudaStreamSynchronize(sd));
-    }
 
     ReadChunk ch;
     ch.n_rec = n_rec;
@@ -378,16 +403,7 @@ void EngineT<NW>::feed_text(const char* text, size_t nbytes, bool on_device, int
     ch.len = reinterpret_cast<u32*>(arena_alloc(n_rec * sizeof(u32)));
     chunks_.push_back(ch);
     t_c = host_now();
-    {
-        const u64 total = n_rec * (u64)W64_;
-        k_decode_fast<<<(unsigned)std::min<u64>((total + 255) / 256, (u64)n_sm_ * 64), 256, 0, sd>>>(d_text, (u64)nbytes, seq_start, seq_end, n_rec, maxlen, W64_,
-                                                                                                 ch.words, ch.len, bad);
-        PG_CUDA(cudaGetLastError());
-        const u64 fix_warps = (n_rec + 31) / 32;
-        k_decode_fix<<<(unsigned)std::min<u64>((fix_warps + 7) / 8, (u64)n_sm_ * 32), 256, 0, sd>>>(d_text, seq_start, seq_end, n_rec, maxlen, reverse_seq, prm_.K, W64_,
-                                                                                              ch.words, ch.len, bad, d_cnt_);
-        PG_CUDA(cudaGetLastError());
-    }
+    decode_records(d_text, nbytes, L, maxlen, reverse_seq, prm_.K, W64_, n_sm_, ch.words, ch.len, d_cnt_, sd);
     PG_CUDA(cudaEventRecord(ev[1], sd));
     if (use_skm) {
         PG_CUDA(cudaEventRecord(ev_dec_done_, sd));

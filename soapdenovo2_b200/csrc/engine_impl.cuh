@@ -95,6 +95,21 @@ static_assert(C_INSTANCES == C_DISTINCT + 1 && C_KEPT == C_DISTINCT + 2, "absorb
 //   Plain      anything else: sweeps() runs k_sweep over the whole table
 enum class PassSweeps { Untouched, Fused, Plain };
 
+// The decode of one text chunk (decode.cu), shared by pass 1 (feed_text) and the map stage (map.cu).  decode_lines counts the
+// records (one host sync of stream sd; h_cnt: pinned, C_COUNT + 1 words) and indexes their sequence lines in line_buf;
+// decode_records packs them into words / lens (W64 words per read) and adds "kmer(s) in reads" / reads kept to d_cnt.
+struct DecodeLines {
+    u32* seq_start;
+    u32* seq_end;
+    u8* bad;
+    u64 n_rec;
+};
+void check_format(const u64* h_cnt);   // throws the malformed-input error when the line index flagged a bad record
+DecodeLines decode_lines(const unsigned char* d_text, size_t nbytes, int fastq, int n_sm, DevBuf& scan_buf, DevBuf& line_buf, u64* d_cnt, u64* h_cnt,
+                         cudaStream_t sd);
+void decode_records(const unsigned char* d_text, size_t nbytes, const DecodeLines& L, int maxlen, int reverse, int K, int W64, int n_sm, u64* words,
+                    u32* lens, u64* d_cnt, cudaStream_t sd);
+
 // The aggregation launch whose outcome (deferred buckets, time) has not been read yet
 struct PendingFlush {
     bool pending = false;

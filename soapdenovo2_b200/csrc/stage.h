@@ -22,6 +22,10 @@ void phase_vertex(IEngine& e, const PgParams& p, const std::string& prefix, pgb2
 struct PlanEntry { std::string path; bool fastq; int mate, reverse, cut; };
 struct ReadPlan { int n_libs, max_rd_len; std::vector<PlanEntry> files; };
 ReadPlan read_plan(const char* cfg);
+// The map stage's plan: every library in config order after the sort by avg_ins, with the files map reads (paired ones, asm_flags 2|3)
+struct MapLib { int avg_ins, reverse, map_len, rank, pair_num_cut; std::vector<PlanEntry> files; };
+struct MapPlan { int max_rd_len; std::vector<MapLib> libs; };
+MapPlan map_plan(const char* cfg);   // refuses asm_flags=4 and b= libraries
 size_t last_record_start(const char* buf, size_t n, bool fastq);   // the chunk cutter
 void write_file(const std::string& name, const void* data, size_t n);
 void write_kmer_freq(const std::string& prefix, const long long hist[256]);

@@ -24,7 +24,7 @@ void fail(const char* fmt, ...) {
 
 namespace {   // the library config (lib.c)
 struct Lib {
-    int avg_ins = 0, asm_flag = 3, reverse = 0, rd_len_cutoff = 0;
+    int avg_ins = 0, asm_flag = 3, reverse = 0, rd_len_cutoff = 0, map_len = 0, rank = 0, pair_num_cut = 0;
     std::vector<std::string> f[7];   // [1]=f1 [0]=f2 [2]=q1 [4]=q2 [3]=p [5]=f [6]=q
 };
 }   // namespace
@@ -60,6 +60,8 @@ static std::vector<Lib> scan_lib(const char* cfg, int* max_rd_len) {
         else if (a == "b") bam = true;
         else if (a == "avg_ins") L.avg_ins = atoi(b.c_str()); else if (a == "reverse_seq") L.reverse = atoi(b.c_str());
         else if (a == "asm_flags") L.asm_flag = atoi(b.c_str()); else if (a == "rd_len_cutoff") L.rd_len_cutoff = atoi(b.c_str());
+        else if (a == "map_len") L.map_len = atoi(b.c_str()); else if (a == "rank") L.rank = atoi(b.c_str());
+        else if (a == "pair_num_cutoff") L.pair_num_cut = atoi(b.c_str());
     }
     fclose(fp);
     if (bam) fail("pgb200: BAM input (b=) is not supported by the GPU engine");
@@ -93,6 +95,29 @@ ReadPlan read_plan(const char* cfg) {
                 } else plan.files.push_back({L.f[type][fi], fq, -1, L.reverse, cut});
             }
         }
+    }
+    return plan;
+}
+
+// The map stage reads with pair = 1 and asm_ctg = 0 (prlRead2Ctg.c:887, readseq1by1.c:595-674): libraries with asm_flags 2|3, and
+// inside each only the f1/f2 pairs, q1/q2 pairs and p files.  Every library is kept for the "LIB(s) information" lines.
+MapPlan map_plan(const char* cfg) {
+    MapPlan plan;
+    const std::vector<Lib> libs = scan_lib(cfg, &plan.max_rd_len);
+    for (const Lib& L : libs) {
+        if (L.asm_flag == 4) fail("pgb200: long-read libraries (asm_flags=4) are not supported by the GPU map stage");
+        MapLib m{L.avg_ins, L.reverse, L.map_len, L.rank, L.pair_num_cut, {}};
+        const int cut = (L.rd_len_cutoff > 0 && L.rd_len_cutoff < plan.max_rd_len) ? L.rd_len_cutoff : plan.max_rd_len;   // readseq1by1.c:1083-1090
+        if (L.asm_flag == 2 || L.asm_flag == 3)
+            for (int type = 1; type <= 3; type++)
+                for (size_t fi = 0; fi < L.f[type].size(); fi++) {
+                    const bool fq = type == 2;
+                    if (type <= 2) {
+                        m.files.push_back({L.f[type][fi], fq, 0, L.reverse, cut});
+                        m.files.push_back({L.f[type == 1 ? 0 : 4][fi], fq, 1, L.reverse, cut});
+                    } else m.files.push_back({L.f[type][fi], fq, -1, L.reverse, cut});
+                }
+        plan.libs.push_back(std::move(m));
     }
     return plan;
 }
