@@ -19,20 +19,25 @@
 #include "engine_impl.cuh"
 #include "skm.cuh"
 #include "scan.cuh"
+#include "chop.cuh"
 
 namespace pgb {
 
 constexpr int SKM_PART_THREADS = 128;
 constexpr int SKM_APPLY_THREADS = 256;
-// Shared-memory table of a bucket: 1024 slots (32 KB at K <= 63) and at most 42 registers per thread put 6 CTAs = 48 warps on an SM
-// (6 x 34 KB of the 228 KB an H100 SM has).  256-bit keys (48 B slots, 78 live registers) stay at 3 CTAs.  These sizes (and the
-// bucket count, skm_init) were chosen on an earlier GPU and have not been re-tuned on H100.
+// Shared-memory table of a bucket: 1024 slots (32 KB at K <= 63) plus the record stage (SKM_STAGE_RECS) put 4 CTAs = 32 warps on an
+// H100 SM (4 x 47 KB of 228 KB) at 64 registers per thread; 256-bit keys (48 B slots, 69 KB per CTA) run 3 CTAs.  On H100 this beat
+// 3 CTAs with a 256-record stage and 4 with a 192-record one (DESIGN.md §5); 5 or 6 CTAs spill at the register budget they allow.
 #ifndef SKM_LOG2_SLOTS
 #define SKM_LOG2_SLOTS 10
 #endif
-#ifndef SKM_APPLY_MIN_BLOCKS
-#define SKM_APPLY_MIN_BLOCKS(NW) ((NW) == 2 ? 6 : 3)
+#ifndef SKM_APPLY_MIN_BLOCKS_NW2
+#define SKM_APPLY_MIN_BLOCKS_NW2 4
 #endif
+#ifndef SKM_APPLY_MIN_BLOCKS_NW4
+#define SKM_APPLY_MIN_BLOCKS_NW4 3
+#endif
+#define SKM_APPLY_MIN_BLOCKS(NW) ((NW) == 2 ? SKM_APPLY_MIN_BLOCKS_NW2 : SKM_APPLY_MIN_BLOCKS_NW4)
 constexpr int SKM_SLOTS = 1 << SKM_LOG2_SLOTS;                       // shared-memory table slots per CTA
 constexpr int SKM_SOFT_LIMIT = SKM_SLOTS - SKM_APPLY_THREADS - 64;   // claims stop here: the table can never fill up completely
 constexpr int SKM_SIDE_RUNS = 16;
@@ -362,25 +367,89 @@ struct SkmApplyArgs {
 };
 constexpr u64 SKM_CREDIT = 1ull << 16;   // table room a CTA reserves at a time (keys)
 
-__device__ __forceinline__ u64 shfl64(u64 v, int src) { return (u64)__shfl_sync(0xffffffffu, (unsigned long long)v, src); }
+// -DSKM_PHASE_CLOCKS: k_skm_apply adds up clock64() per phase over all its threads (stage wait, instance build, find / claim, apply,
+// spill to the global table, flush); the host prints the totals of every aggregation with PGB200_SKM_STATS.  Off: no code at all.
+#ifdef SKM_PHASE_CLOCKS
+constexpr int SKM_PHASES = 6;
+__device__ unsigned long long g_skm_phase_clk[SKM_PHASES];
+#define SKM_T0(v) const long long v = clock64()
+#define SKM_ACC(i, v) clk[i] += (u64)(clock64() - (v))
+#else
+#define SKM_T0(v)
+#define SKM_ACC(i, v)
+#endif
 
-// One CTA per bucket (static round-robin over the list: buckets are hash-uniform), one shared-memory table per CTA.  Inside a bucket
-// the WARPS run on their own: a warp loads 32 consecutive records of the bucket (one 32 / 48 B record per lane, coalesced), an
-// inclusive scan of their k-mer counts maps instance q of the batch to (record, position), and every warp step takes 32 CONSECUTIVE
-// instances -- all lanes busy whatever the run lengths -- fetching its record from the lane that holds it with shuffles.  No CTA-wide
-// barrier and no staging buffer inside a bucket; the next batch's records and the next bucket's segment ranges are loaded while the
-// current ones are processed.
+// Exclusive prefix sum over the CTA; *total = the sum.  The caller separates two calls with a __syncthreads (s_warp is reused).
+__device__ __forceinline__ u32 cta_exclusive_scan(u32 v, u32* s_warp, u32& total) {
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    u32 inc = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const u32 u = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc += u;
+    }
+    if (lane == 31) s_warp[wid] = inc;
+    __syncthreads();
+    u32 off = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < SKM_APPLY_THREADS / 32; w++) {
+        const u32 s = s_warp[w];
+        off += w < wid ? s : 0u;
+        tot += s;
+    }
+    total = tot;
+    return off + inc - v;
+}
+
+// Records of one bucket staged per window: the window is W consecutive records of the bucket's concatenated segment ranges; every
+// segment thread copies its part of the window with one bulk copy, completed on the half's mbarrier.  The stage is double-buffered:
+// the next window (or the next bucket's first) is in flight while the current one is processed, flushed and synchronised.
+#ifndef SKM_STAGE_RECS
+#define SKM_STAGE_RECS 128
+#endif
+constexpr int SKM_W = SKM_STAGE_RECS;
+static_assert(SKM_W <= SKM_APPLY_THREADS, "the per-record pre-pass runs one thread per staged record");
+
+// A segment thread's part of one bucket: records lo .. lo+cnt-1 of its segment, at positions cum .. cum+cnt-1 of the bucket.
+struct SkmSegRange {
+    u32 lo, cnt, cum;
+};
+// Queue window w of a bucket of R records into a stage half.  Every thread calls it: thread 0 arrives with the window's byte count,
+// the segment threads whose range meets the window copy their part.
+template <int RW>
+__device__ __forceinline__ void skm_stage_window(u64* stage, u64* bar, const u64* my_recs, const SkmSegRange& sr, u32 R, u32 w) {
+    const u32 a = w * (u32)SKM_W, e = min(R, a + (u32)SKM_W);
+    if (threadIdx.x == 0) mbar_expect_tx(bar, (e - a) * (u32)(RW * sizeof(u64)));
+    if (my_recs) {
+        const u32 s0 = max(sr.cum, a), s1 = min(sr.cum + sr.cnt, e);
+        if (s0 < s1) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic reads of this half come first
+            tma_bulk_g2s(stage + (u64)(s0 - a) * RW, my_recs + (u64)(sr.lo + s0 - sr.cum) * RW, (s1 - s0) * (u32)(RW * sizeof(u64)), bar);
+        }
+    }
+}
+
+// One CTA per bucket (static round-robin over the list: buckets are hash-uniform), one shared-memory table per CTA.  A bucket is
+// processed window by window (skm_stage_window); the table persists over the windows and is flushed once per bucket.  When a window
+// has landed, one thread per record writes its k-mer count prefix P and its reversed bases (skm_rec_reverse) next to the stage.  The
+// warps then split the window's instances into contiguous slices and take 32 CONSECUTIVE instances per step -- all lanes busy
+// whatever the run lengths: the records that start inside the step come from one lookahead load of P, and every lane builds its
+// k-mer and reverse complement with two shifts of shared-memory words (skm_instance_staged).
 template <int NW>
 __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k_skm_apply(Table<NW> tab, KParams<NW> kp, SkmApplyArgs a) {
     constexpr int RW = NW + 2, WARPS = SKM_APPLY_THREADS / 32;
-    extern __shared__ __align__(16) u64 s_dyn[];   // key[NW][S], pay[S], rnk[S], list[S] (u16)
-    __shared__ const u64* s_ptr[SKM_MAX_SEGS];
-    __shared__ u32 s_cum[SKM_MAX_SEGS + 1];
+    // key[NW][S], pay[S], rnk[S], stage[2][W][RW], rv[W][NW+1], list[S] (u16), P[W+1]
+    extern __shared__ __align__(16) u64 s_dyn[];
+    u64* const s_stage = s_dyn + (NW + 2) * SKM_SLOTS;
+    u64* const s_rv = s_stage + 2 * SKM_W * RW;
+    unsigned short* const s_list = reinterpret_cast<unsigned short*>(s_rv + SKM_W * (NW + 1));
+    u32* const s_P = reinterpret_cast<u32*>(s_list + SKM_SLOTS);
+    __shared__ __align__(8) u64 s_bar[2];
     __shared__ u32 s_warp[WARPS];
-    __shared__ u32 s_count, s_defer, s_batch;
+    __shared__ u32 s_count, s_defer;
     __shared__ unsigned s_new, s_tot_new;
     __shared__ SweepTally s_sw;   // the fused sweeps (a.sweep)
-    SmemTable<NW, SKM_SLOTS, SKM_SOFT_LIMIT, unsigned short> st{s_dyn, s_dyn + NW * SKM_SLOTS, s_dyn + (NW + 1) * SKM_SLOTS, reinterpret_cast<unsigned short*>(s_dyn + (NW + 2) * SKM_SLOTS), &s_count};
+    SmemTable<NW, SKM_SLOTS, SKM_SOFT_LIMIT, unsigned short> st{s_dyn, s_dyn + NW * SKM_SLOTS, s_dyn + (NW + 1) * SKM_SLOTS, s_list, &s_count};
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const unsigned lane_le = 0xffffffffu >> (31 - lane);
     for (int i = tid; i < SKM_SLOTS; i += SKM_APPLY_THREADS) {   // the flush re-empties what it merges
@@ -388,7 +457,11 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         st.pay[i] = PAYLOAD_FRESH;
         st.rnk[i] = ~0ull;
     }
-    if (tid == 0) s_tot_new = 0;
+    if (tid == 0) {
+        s_tot_new = 0;
+        mbar_init(&s_bar[0], 1);
+        mbar_init(&s_bar[1], 1);
+    }
     static_assert(SKM_APPLY_THREADS == 256, "one histogram bin per thread");
     s_sw.clear();
     unsigned sw_lin = 0, sw_rem = 0;
@@ -397,39 +470,33 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     const u64* my_recs = tid < n_segs ? a.segs->recs[tid] : nullptr;
     unsigned tot_new = 0;
     u64 credit = 0;                      // thread 0: table room this CTA holds
+#ifdef SKM_PHASE_CLOCKS
+    u64 clk[SKM_PHASES] = {};
+#endif
+    auto seg_range = [&](u32 p, SkmSegRange& r) {   // this thread's range of the bucket at list position p (empty past the list)
+        r.lo = r.cnt = 0;
+        if (p < a.n_list && my_so) {
+            const u32 b = a.bucket_list ? a.bucket_list[p] : p;
+            r.lo = my_so[b];
+            r.cnt = my_so[b + 1] - r.lo;
+        }
+    };
     u32 pos = blockIdx.x;
-    u32 nlo = 0, ncnt = 0;               // this thread's segment range of the NEXT bucket
-    if (pos < a.n_list && my_so) {
-        const u32 b = a.bucket_list ? a.bucket_list[pos] : pos;
-        nlo = my_so[b];
-        ncnt = my_so[b + 1] - nlo;
-    }
+    SkmSegRange cur, nxt, nn;            // this thread's ranges of the current, the next and the one after
+    seg_range(pos, cur);
+    seg_range(pos + gridDim.x, nxt);
+    u32 R_cur;
+    cur.cum = cta_exclusive_scan(cur.cnt, s_warp, R_cur);
+    unsigned half = 0, phase = 0;        // stage half of the current window; bit h: parity of half h's next completion
+    __syncthreads();                     // the mbarriers are initialised
+    if (pos < a.n_list) skm_stage_window<RW>(s_stage, &s_bar[0], my_recs, cur, R_cur, 0);
     for (; pos < a.n_list; pos += gridDim.x) {
         __syncthreads();   // previous bucket fully flushed (and the empty table visible on the first trip)
-        const u32 cnt = ncnt;
-        if (my_so) s_ptr[tid] = my_recs + (u64)nlo * RW;
-        if (tid == 0) { s_count = 0; s_new = 0; s_batch = WARPS; }
-        if (pos + gridDim.x < a.n_list && my_so) {
-            const u32 nb = a.bucket_list ? a.bucket_list[pos + gridDim.x] : pos + gridDim.x;
-            nlo = my_so[nb];
-            ncnt = my_so[nb + 1] - nlo;
-        }
-        {
-            u32 inc = cnt;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const u32 v = __shfl_up_sync(0xffffffffu, inc, d);
-                if (lane >= d) inc += v;
-            }
-            if (lane == 31) s_warp[wid] = inc;
-            __syncthreads();
-            u32 off = 0;
-            for (int w = 0; w < wid; w++) off += s_warp[w];
-            if (tid < n_segs) s_cum[tid] = off + inc - cnt;
-            if (tid == (n_segs > 0 ? n_segs - 1 : 0)) s_cum[n_segs] = n_segs > 0 ? off + inc : 0u;
-        }
-        __syncthreads();
-        const u32 R = s_cum[n_segs];
+        u32 R_nxt;
+        nxt.cum = cta_exclusive_scan(nxt.cnt, s_warp, R_nxt);
+        seg_range(pos + 2 * gridDim.x, nn);
+        if (tid == 0) { s_count = 0; s_new = 0; }
+        const u32 R = R_cur;
         // ---- room in the global table: every k-mer instance could be a new key.  Credits are taken SKM_CREDIT keys at a time.
         if (tid == 0) {
             bool defer = false;
@@ -459,106 +526,100 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             s_defer = defer ? 1u : 0u;
         }
         __syncthreads();
-        if (s_defer || R == 0) {
-            if (tid == 0 && !s_defer) credit += (u64)R * SKM_MAX_RUN;
-            continue;
-        }
+        const bool run = !s_defer && R > 0;
         unsigned my_new = 0;
-        // ---- the warps: batches of 32 records, 32 consecutive instances per step
-        u64 nh = 0, nx[NW + 1];
+        // ---- the windows of the bucket (a deferred or empty bucket still retires the window queued for it)
+        for (u32 w = 0;; w++) {
+            const bool more = run && (w + 1) * (u32)SKM_W < R;
+            if (more) skm_stage_window<RW>(s_stage + (half ^ 1) * SKM_W * RW, &s_bar[half ^ 1], my_recs, cur, R, w + 1);
+            else if (pos + gridDim.x < a.n_list) skm_stage_window<RW>(s_stage + (half ^ 1) * SKM_W * RW, &s_bar[half ^ 1], my_recs, nxt, R_nxt, 0);
+            SKM_T0(t_wait);
+            mbar_wait(&s_bar[half], (phase >> half) & 1u);
+            SKM_ACC(0, t_wait);
+            phase ^= 1u << half;
+            if (run) {
+                SKM_T0(t_pre);
+                const u64* stg = s_stage + half * SKM_W * RW;
+                const u32 nrec = min(R - w * (u32)SKM_W, (u32)SKM_W);
+                // per record: its k-mer count prefix and its reversed bases
+                u32 n = 0;
+                if ((u32)tid < nrec) {
+                    const u64 hdr = stg[tid * RW];
+                    n = (u32)skm_rec_n(hdr);
+                    u64 rv[NW + 1];
+                    skm_rec_reverse<NW>(hdr, stg + tid * RW + 1, rv, kp.K);
 #pragma unroll
-        for (int i = 0; i < NW + 1; i++) nx[i] = 0;
-        // batch size: the bucket's records are split evenly over a multiple of WARPS batches (R = 210 records on 8 warps: 8 batches of
-        // 27, not 6 of 32 + 1 of 18 + an idle warp), so the warps reach the barrier before the flush together
-        const u32 n_batches = (u32)WARPS * ((R + 32u * WARPS - 1) / (32u * WARPS));
-        const u32 bsz = (R + n_batches - 1) / n_batches;   // <= 32
-        auto load_rec = [&](u32 q) {
-            nh = 0;
-            if (q < R && lane < (int)bsz) {
-                int lo = 0, hi = n_segs;
-                while (hi - lo > 1) {
-                    const int mid = (lo + hi) >> 1;
-                    if (s_cum[mid] <= q) lo = mid; else hi = mid;
+                    for (int i = 0; i < NW + 1; i++) s_rv[tid * (NW + 1) + i] = rv[i];
                 }
-                const uint4* p = reinterpret_cast<const uint4*>(s_ptr[lo] + (u64)(q - s_cum[lo]) * RW);
-                u64 w[RW];
-#pragma unroll
-                for (int i = 0; i < RW / 2; i++) {
-                    const uint4 v = __ldg(p + i);
-                    w[2 * i] = (u64)v.x | ((u64)v.y << 32);
-                    w[2 * i + 1] = (u64)v.z | ((u64)v.w << 32);
+                u32 I;
+                const u32 p = cta_exclusive_scan(n, s_warp, I);
+                if ((u32)tid < nrec) s_P[tid] = p;
+                if (tid == 0) s_P[nrec] = I;
+                __syncthreads();
+                SKM_ACC(1, t_pre);
+                // ---- the warps: contiguous slices of the window's instances, 32 consecutive instances per step
+                const u32 steps = (I + 31) / 32, per = (steps + WARPS - 1) / WARPS;
+                const u32 q_end = min(I, (wid + 1) * per * 32);
+                u32 q0 = wid * per * 32;
+                u32 r0 = 0;   // the record holding q0: the last record with P <= q0
+                if (q0 < q_end) {
+                    u32 lo = 0, hi = nrec;
+                    while (hi - lo > 1) {
+                        const u32 mid = (lo + hi) >> 1;
+                        if (s_P[mid] <= q0) lo = mid; else hi = mid;
+                    }
+                    r0 = lo;
                 }
-                nh = w[0];
-#pragma unroll
-                for (int i = 0; i < NW + 1; i++) nx[i] = w[1 + i];
-            }
-        };
-        // batches are handed out dynamically (the first WARPS ones are pre-assigned): a warp that draws short runs takes more of them,
-        // so the warps reach the barrier before the flush together
-        load_rec((u32)wid * bsz + lane);
-        u32 nb = 0x7FFFFFFu;                                  // (a warp without a first batch must not draw one; x 32 still fits)
-        if ((u32)wid * bsz < R) {
-            if (lane == 0) nb = atomicAdd(&s_batch, 1u);
-            nb = __shfl_sync(0xffffffffu, nb, 0);
-        }
-        for (u32 rb = (u32)wid * bsz; rb < R;) {
-            const u64 hdr = nh;
-            u64 x[NW + 1];
-#pragma unroll
-            for (int i = 0; i < NW + 1; i++) x[i] = nx[i];
-            const u32 rb_next = nb * bsz;
-            load_rec(rb_next + lane);                         // the next batch is in flight while this one is processed
-            if (rb_next < R) {
-                if (lane == 0) nb = atomicAdd(&s_batch, 1u);
-                nb = __shfl_sync(0xffffffffu, nb, 0);
-            }
-            const bool valid = rb + lane < R && lane < (int)bsz;
-            const u32 n = valid ? (u32)skm_rec_n(hdr) : 0u;
-            u32 inc = n;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const u32 v = __shfl_up_sync(0xffffffffu, inc, d);
-                if (lane >= d) inc += v;
-            }
-            const u32 I = __shfl_sync(0xffffffffu, inc, 31);
-            const u32 pe = inc - n;                            // first instance of this lane's record inside the batch
-            for (u32 q0 = 0; q0 < I; q0 += 32) {
-                const u32 q = q0 + lane;
-                const bool has = q < I;
-                // record of instance q: the record that holds q0, plus the records that start at window positions 1 .. lane
-                const unsigned starts = __reduce_or_sync(0xffffffffu, (valid && pe > q0 && pe - q0 < 32u) ? 1u << (pe - q0) : 0u);
-                const int first = __popc(__ballot_sync(0xffffffffu, valid && pe <= q0)) - 1;
-                const int src = (first + __popc(starts & lane_le)) & 31;
-                const int t = (int)(q - __shfl_sync(0xffffffffu, pe, src));
-                const u64 h = shfl64(hdr, src);
-                u64 y[NW + 1];
-#pragma unroll
-                for (int i = 0; i < NW + 1; i++) y[i] = shfl64(x[i], src);
-                const unsigned has_mask = __ballot_sync(0xffffffffu, has);
-                if (has) {
-                    const SkmInst<NW> in = skm_instance_rec<NW>(kp, h, y, t);
-                    const u64 rank = skm_rec_rank(h, t);
-                    u32 slot;
-                    const int state = st.find(tab, in.canon, slot);
-                    __syncwarp(has_mask);   // the lanes re-join before the counter update (see SmemTable)
-                    if (state == 1) st.apply(slot, in.left, in.right, rank);
-                    else if (state == 3) {
-                        // bucket holds more distinct k-mers than the shared-memory table: this instance goes to HBM directly (same result)
-                        u64 at;
-                        const bool fresh = table_insert(tab, in.canon, in.left, in.right, rank, &at);
-                        my_new += fresh;
-                        if (fresh && a.sweep) {   // its other instances follow the same way: swept after the launch, from this list
-                            const u64 n = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
-                            if (n < a.spill_cap) a.spill_list[n] = at;
+                for (; q0 < q_end; q0 += 32) {
+                    const u32 q = q0 + lane;
+                    const bool has = q < q_end;
+                    SKM_T0(t_inst);
+                    // the records that start at step positions 1 .. 31 (P is strictly increasing: every record holds a k-mer)
+                    const u32 pn = s_P[min(r0 + 1 + lane, nrec)];
+                    const unsigned starts = __reduce_or_sync(0xffffffffu, pn - q0 - 1 < 31u ? 1u << (pn - q0) : 0u);
+                    const u32 rec = r0 + __popc(starts & lane_le);
+                    r0 += __popc(__ballot_sync(0xffffffffu, pn <= q0 + 32));
+                    const unsigned has_mask = __ballot_sync(0xffffffffu, has);
+                    if (has) {
+                        const int t = (int)(q - s_P[rec]);
+                        const u64 h = stg[rec * RW];
+                        const SkmInst<NW> in = skm_instance_staged<NW>(kp, h, stg + rec * RW + 1, s_rv + rec * (NW + 1), t);
+                        const u64 rank = skm_rec_rank(h, t);
+                        SKM_ACC(1, t_inst);
+                        SKM_T0(t_find);
+                        u32 slot;
+                        const int state = st.find(tab, in.canon, slot);
+                        __syncwarp(has_mask);   // the lanes re-join before the counter update (see SmemTable)
+                        SKM_ACC(2, t_find);
+                        SKM_T0(t_upd);
+                        if (state == 1) {
+                            st.apply(slot, in.left, in.right, rank);
+                            SKM_ACC(3, t_upd);
+                        } else if (state == 3) {
+                            // bucket holds more distinct k-mers than the shared-memory table: this instance goes to HBM directly (same result)
+                            u64 at;
+                            const bool fresh = table_insert(tab, in.canon, in.left, in.right, rank, &at);
+                            my_new += fresh;
+                            if (fresh && a.sweep) {   // its other instances follow the same way: swept after the launch, from this list
+                                const u64 sn = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
+                                if (sn < a.spill_cap) a.spill_list[sn] = at;
+                            }
+                            SKM_ACC(4, t_upd);
                         }
                     }
+                    __syncwarp();
                 }
-                __syncwarp();
             }
-            rb = rb_next;
+            __syncthreads();   // the window's stage half, P and rv are free again
+            half ^= 1;
+            if (!more) break;
         }
-        __syncthreads();
+        cur = nxt;
+        nxt = nn;
+        R_cur = R_nxt;
+        if (!run) continue;
         // ---- flush: one global update per distinct k-mer of the bucket, walking the claim list (every thread busy)
+        SKM_T0(t_flush);
         const u32 n_claimed = s_count;
         for (u32 i = tid; i < n_claimed; i += SKM_APPLY_THREADS) {
             const u32 idx = st.list[i];
@@ -577,6 +638,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         if (my_new) atomicAdd(&s_new, my_new);
         tot_new += my_new;
         __syncthreads();
+        SKM_ACC(5, t_flush);
         if (tid == 0) credit += (u64)R * SKM_MAX_RUN - (u64)s_new;   // what the bound over-reserved stays with the CTA
     }
     __syncthreads();
@@ -584,12 +646,16 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     if (tot_new) atomicAdd(&s_tot_new, tot_new);
     s_sw.flush(sw_lin, sw_rem, a.hist, &a.counters[C_LINEAR], &a.counters[C_REMOVED]);   // (all zero without a.sweep)
     if (tid == 0 && s_tot_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_tot_new);
+#ifdef SKM_PHASE_CLOCKS
+    for (int i = 0; i < SKM_PHASES; i++) atomicAdd(&g_skm_phase_clk[i], (unsigned long long)clk[i]);
+#endif
 }
 
 // ------------------------------------------------------------------------------------------------ host side
 template <int NW>
 static constexpr size_t skm_apply_smem() {
-    return (size_t)(NW + 2) * SKM_SLOTS * sizeof(u64) + (size_t)SKM_SLOTS * sizeof(unsigned short);
+    return ((size_t)(NW + 2) * SKM_SLOTS + 2 * SKM_W * (NW + 2) + SKM_W * (NW + 1)) * sizeof(u64) + (size_t)SKM_SLOTS * sizeof(unsigned short) +
+           (SKM_W + 1) * sizeof(u32);
 }
 // An aggregation launch keeps the keys the table is committed to under this share of its capacity (buckets beyond it are deferred),
 // and the growth before their re-run leaves this much HBM free
@@ -771,7 +837,8 @@ void EngineT<NW>::skm_make_room(u64 n_rec, bool host_text) {
     if (xa_geom_.world == 1) {
         // Host text arrives at PCIe speed and leaves the GPU idle most of the time: whenever the insert stream has drained and at least
         // two chunks are waiting, they are aggregated right away, so that only the last couple of chunks remain for pgb200_finish_pass1.
-        // Device-resident text is fed faster than it is partitioned: the stream never drains and everything is aggregated once.
+        // Device-resident text is fed faster than it is partitioned: the stream never drains and everything is aggregated once, unless
+        // the arena really fills up.
         // PGB200_SKM_FLUSH_EVERY=n forces a fixed cadence (0: only when the arena is full).
         bool early = false;
         if (skm_flush_every_ > 0) early = xa_seg_idx_ >= (u32)skm_flush_every_;
@@ -779,7 +846,14 @@ void EngineT<NW>::skm_make_room(u64 n_rec, bool host_text) {
             early = cudaStreamQuery(st_) == cudaSuccess;
             if (!early) cudaGetLastError();   // cudaErrorNotReady is not an error; do not leave it for the next launch check
         }
-        const bool full = xa_seg_idx_ >= xa_geom_.max_seg || skm_room_estimate(n_rec) > xa_geom_.cap_pair;
+        bool full = xa_seg_idx_ >= xa_geom_.max_seg || skm_room_estimate(n_rec) > xa_geom_.cap_pair;
+        if (full && !early && xa_seg_idx_ < xa_geom_.max_seg && !(h_cnt_[C_XEPOCH] == xa_send_epoch_ + 1 && h_cnt_[C_XSEGS] >= xa_seg_idx_)) {
+            // The estimate ran on counters that lag the partition stream (at worst on the first-chunk guess, several times the records
+            // a read really makes).  A flush costs a pass over every owned bucket and a merge per distinct k-mer per flush, so wait for
+            // the chunks already queued (this chunk's decode keeps running on its own stream) and decide on what they really made.
+            read_counters_on(st_);
+            full = skm_room_estimate(n_rec) > xa_geom_.cap_pair;
+        }
         if ((full || early) && xa_seg_idx_ > 0) {
             skm_close_epoch(false);
             skm_flush();
@@ -948,6 +1022,17 @@ void EngineT<NW>::skm_flush_complete() {
     if (prm_.verbose >= 2 || getenv("PGB200_SKM_STATS"))
         fprintf(stderr, "[pgb200] aggregated epoch %llu: %u owned bucket(s), %d launch(es), %.2f ms, table %llu slots\n", (unsigned long long)xa_flushed_epoch_,
                 skm_own_hi_ - skm_own_lo_, launches, ms, (unsigned long long)cap_);
+#ifdef SKM_PHASE_CLOCKS
+    if (getenv("PGB200_SKM_STATS")) {
+        unsigned long long c[SKM_PHASES], zero[SKM_PHASES] = {}, tot = 0;
+        PG_CUDA(cudaMemcpyFromSymbol(c, g_skm_phase_clk, sizeof(c)));
+        PG_CUDA(cudaMemcpyToSymbol(g_skm_phase_clk, zero, sizeof(zero)));
+        for (int i = 0; i < SKM_PHASES; i++) tot += c[i];
+        fprintf(stderr, "[pgb200] aggregation phase clocks (thread-cycles, %% of %.3g): stage wait %.1f, instance build %.1f, find/claim %.1f, apply %.1f, "
+                        "spill %.1f, flush %.1f\n", (double)tot, 100.0 * c[0] / tot, 100.0 * c[1] / tot, 100.0 * c[2] / tot, 100.0 * c[3] / tot, 100.0 * c[4] / tot,
+                100.0 * c[5] / tot);
+    }
+#endif
 }
 
 template <int NW>

@@ -256,6 +256,74 @@ PG_HD SkmInst<NW> skm_instance_rec(const KParams<NW>& kp, u64 hdr, const u64 (&x
     return r;
 }
 
+// The same instances from a record staged in shared memory (skm.cu stages a window of records at a time).  Once per record the
+// aggregation writes rv[0..NW]: the record's bases 0 .. n+K-1 in REVERSE order, base n+K-1 at bit 0 and base p at bit 2(n+K-1-p)
+// (the right neighbour of the last k-mer is dropped).  Forward k-mer t is then rv >> 2(n-1-t), a shift by less than 64 bits like the
+// one that gives the reverse complement from the record words: no per-instance reverse complement.
+template <int NW, int WS>
+PG_HD void skm_rev_shift(const u64* x, u64 (&rv)[NW + 1], int bs) {
+#pragma unroll
+    for (int i = 0; i < NW + 1; i++) {   // word j of the reversed record is rev2bit64(x[NW - j])
+        const u64 lo = i + WS <= NW ? rev2bit64(x[i + WS <= NW ? NW - i - WS : 0]) : 0ull;
+        const u64 hi = i + WS + 1 <= NW ? rev2bit64(x[i + WS + 1 <= NW ? NW - i - WS - 1 : 0]) : 0ull;
+        rv[i] = bs ? ((lo >> bs) | (hi << (64 - bs))) : lo;
+    }
+}
+template <int NW>
+PG_HD void skm_rec_reverse(u64 hdr, const u64* x, u64 (&rv)[NW + 1], int K) {
+    // all 32(NW+1) bases reversed (base p at bit 2(32(NW+1)-1-p)), shifted right by s; 2 <= s since n + K <= 32(NW+1) - 1.  The word
+    // offset goes through a switch so that every index is a constant (a dynamically indexed array lives in local memory on the GPU).
+    const int s = 2 * (32 * (NW + 1) - skm_rec_n(hdr) - K), bs = s & 63;
+    switch (s >> 6) {
+        case 0: skm_rev_shift<NW, 0>(x, rv, bs); break;
+        case 1: skm_rev_shift<NW, 1>(x, rv, bs); break;
+        case 2: skm_rev_shift<NW, 2>(x, rv, bs); break;
+        case 3: skm_rev_shift<NW, (NW > 2 ? 3 : 2)>(x, rv, bs); break;
+        default: skm_rev_shift<NW, (NW > 2 ? 4 : 2)>(x, rv, bs); break;
+    }
+}
+// k-mer t of a record: hdr, base words x[0..NW] (x[i] = rec.w[1 + i]) and rv[0..NW] from skm_rec_reverse.  Equals skm_instance_rec.
+template <int NW>
+PG_HD SkmInst<NW> skm_instance_staged(const KParams<NW>& kp, u64 hdr, const u64* x, const u64* rv, int t) {
+    const int K = kp.K;
+    const int sh = 2 * t;                             // 0 .. 62
+    const int sf = 2 * (skm_rec_n(hdr) - 1 - t);      // 0 .. 62
+    u64 y[NW + 1], v[NW + 1];                         // bases t .. from bit 0; the reversed bases from base t+K down
+#pragma unroll
+    for (int i = 0; i < NW + 1; i++) { y[i] = x[i]; v[i] = rv[i]; }
+#pragma unroll
+    for (int i = 0; i < NW + 1; i++) {
+        const u64 hy = i + 1 < NW + 1 ? y[i + 1] : 0ull, hv = i + 1 < NW + 1 ? v[i + 1] : 0ull;
+        y[i] = sh ? ((y[i] >> sh) | (hy << (64 - sh))) : y[i];
+        v[i] = sf ? ((v[i] >> sf) | (hv << (64 - sf))) : v[i];
+    }
+    const unsigned pv = (t > 0 || skm_rec_has_prev(hdr)) ? (unsigned)(y[0] & 3) : 4u;
+    u64 z[NW];              // bases t+1 .. from bit 0: the k-mer, then its right neighbour at bit 2K
+#pragma unroll
+    for (int i = 0; i < NW; i++) z[i] = (y[i] >> 2) | (y[i + 1] << 62);
+    unsigned cn = 4;
+    if (!(skm_rec_last(hdr) && t == skm_rec_n(hdr) - 1)) {
+        const int bit = 2 * K, wi = bit >> 6;
+        u64 c = 0;
+#pragma unroll
+        for (int i = 0; i < NW; i++)
+            if (i == wi) c = z[i];
+        cn = (unsigned)((c >> (bit & 63)) & 3);
+    }
+    Kmer<NW> rc, fwd;
+#pragma unroll
+    for (int i = 0; i < NW; i++) {
+        rc.w[NW - 1 - i] = (z[i] ^ 0xAAAAAAAAAAAAAAAAull) & kp.mask.w[NW - 1 - i];
+        fwd.w[NW - 1 - i] = v[i] & kp.mask.w[NW - 1 - i];
+    }
+    SkmInst<NW> r;
+    const bool sm = kless(fwd, rc);          // KmerSmaller(word, bal_word); tie -> rc branch
+    r.canon = sm ? fwd : rc;
+    r.left = sm ? pv : (cn < 4 ? (cn ^ 2u) : 4u);
+    r.right = sm ? cn : (pv < 4 ? (pv ^ 2u) : 4u);
+    return r;
+}
+
 // ---------------------------------------------------------------- lane packing
 // P[0..nt] = exclusive prefix sums of the k-mer counts of a tile of nt records.  Instance q of the tile belongs to the last record r
 // with P[r] <= q (every record holds at least one k-mer, so P is strictly increasing); its position inside the record is q - P[r].
