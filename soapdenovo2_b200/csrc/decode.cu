@@ -8,8 +8,10 @@
 //   k_line_index  line number of every newline from the scanned tile counts -> start/end of every sequence line; checks that
 //                 header lines start with '>' / '@' and FASTQ separator lines with '+'          (1 x text)
 //   k_decode_fast one thread per 32-base output word: 36 bytes of text -> 64 packed bits with SIMD-in-register byte arithmetic
-//                 (0.5 x text); records that need the general rules (a byte that is not a letter inside the line, reverse_seq) are
-//                 flagged and redone by k_decode_fix, one warp per flagged record, which also accumulates the read statistics.
+//                 (0.5 x text); it also adds up the read statistics.  A record that needs the general rules (a byte that is not a
+//                 letter inside the line) is appended once to a redo list; k_decode_fix, on a small fixed grid, redoes just the
+//                 listed records (every record of a reverse_seq library), one warp per record, and corrects their statistics.  On
+//                 clean text the list is empty and k_decode_fix returns at once.
 // Base code = (ch & 6) >> 1 for letters (A0 C1 T2 G3, N->3), '.' -> 0, every other byte is dropped; only the first
 // min(linelen, maxlen) characters of the sequence line are considered (readseq1by1.c:177-200).  Output: LSB-first 2-bit packing,
 // W64 words per read, zero past the read's end.
@@ -172,10 +174,28 @@ __device__ __forceinline__ unsigned base_char_mask4(unsigned v, unsigned& dot) {
     return (__vcmpgeu4(t, 0x61616161u) & __vcmpleu4(t, 0x7A7A7A7Au)) | dot;
 }
 
+// "kmer(s) in reads" / reads kept of a read of n bases: reads shorter than K+1 are skipped (prlHashReads.c:504,642)
+__device__ __forceinline__ u64 read_instances(int n, int K) { return n >= K + 1 ? (u64)(n - K + 1) : 0ull; }
+
+// Sum of v over the CTA, added to *dst with one global atomic (every thread of the CTA calls it)
+__device__ __forceinline__ void cta_add_u64(u64 v, u64* dst) {
+    __shared__ u64 s_sum;
+    if (threadIdx.x == 0) s_sum = 0;
+    __syncthreads();
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_down_sync(0xffffffffu, v, d);
+    if ((threadIdx.x & 31) == 0 && v) atomicAdd((unsigned long long*)&s_sum, (unsigned long long)v);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_sum) atomicAdd((unsigned long long*)dst, (unsigned long long)s_sum);
+}
+
+// Every record is counted here with the length of its fast decode; a record the fast rules cannot handle is appended (once) to the
+// redo list, and k_decode_fix corrects the counters of just those records.
 __global__ void __launch_bounds__(256) k_decode_fast(const unsigned char* __restrict__ text, u64 nbytes, const u32* __restrict__ seq_start,
-                                                     const u32* __restrict__ seq_end, u64 n_rec, int maxlen, int W64, u64* __restrict__ words,
-                                                     u32* __restrict__ lens, u8* __restrict__ bad) {
+                                                     const u32* __restrict__ seq_end, u64 n_rec, int maxlen, int K, int W64, u64* __restrict__ words,
+                                                     u32* __restrict__ lens, u32* __restrict__ flag, u32* __restrict__ redo, u32* n_redo, u64* counters) {
     const u64 total = n_rec * (u64)W64;
+    u64 inst = 0, kept = 0;
     for (u64 idx = (u64)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (u64)gridDim.x * blockDim.x) {
         const u64 r = idx / (unsigned)W64;
         const int w = (int)(idx - r * (unsigned)W64);
@@ -183,7 +203,12 @@ __global__ void __launch_bounds__(256) k_decode_fast(const unsigned char* __rest
         const int raw = e > s ? (int)min(e - s, 0x7fffffffu) : 0;
         int use = raw < maxlen ? raw : maxlen;
         if (raw > 0 && raw <= maxlen && text[e - 1] == '\r') use = raw - 1;   // CRLF: the '\r' would be dropped as a non-letter
-        if (w == 0) { lens[r] = (u32)use; }
+        if (w == 0) {
+            lens[r] = (u32)use;
+            const u64 n = read_instances(use, K);
+            inst += n;
+            kept += n ? 1 : 0;
+        }
         int cnt = use - 32 * w;
         if (cnt <= 0) { words[idx] = 0ull; continue; }
         if (cnt > 32) cnt = 32;
@@ -202,23 +227,26 @@ __global__ void __launch_bounds__(256) k_decode_fast(const unsigned char* __rest
             const unsigned v = __funnelshift_r(t[i], t[i + 1], sh);
             int nb = cnt - 4 * i;
             nb = nb < 0 ? 0 : (nb > 4 ? 4 : nb);
-            const unsigned need = nb == 4 ? 0xFFFFFFFFu : ((1u << (8 * nb)) - 1u);
+            const unsigned need = (unsigned)((1ull << (8 * nb)) - 1ull);   // nb in 0..4: a 64-bit shift is defined for all of them
             unsigned dot;
             const unsigned ok = base_char_mask4(v, dot);
             clean = clean && ((ok & need) == need);
             const unsigned codes = ((v >> 1) & 0x03030303u) & ~dot & need;
             out |= (u64)((codes * 0x01041040u) >> 24) << (8 * i);   // 4 two-bit codes, one per byte -> one byte
         }
-        if (!clean) bad[r] = 1;
+        if (!clean && atomicOr(&flag[r], 1u) == 0u) redo[atomicAdd(n_redo, 1u)] = (u32)r;
         words[idx] = out;
     }
+    cta_add_u64(inst, &counters[C_INSTANCES]);
+    cta_add_u64(kept, &counters[C_KEPT]);
 }
 
 __device__ __forceinline__ bool is_base_char(unsigned c) { return ((c | 0x20u) - 'a') < 26u || c == '.'; }
 __device__ __forceinline__ unsigned base_code(unsigned c) { return c == '.' ? 0u : ((c & 6u) >> 1); }
 
-// general rules, one warp per record: drop every byte that is not a letter or '.', optional whole-read reverse complement
-__device__ void decode_record_warp(const unsigned char* __restrict__ text, u32 s, u32 e, int maxlen, int reverse, int W64, u64* out, u32* len_out) {
+// general rules, one warp per record: drop every byte that is not a letter or '.', optional whole-read reverse complement; returns the
+// read's length (warp-uniform)
+__device__ int decode_record_warp(const unsigned char* __restrict__ text, u32 s, u32 e, int maxlen, int reverse, int W64, u64* out, u32* len_out) {
     const int lane = threadIdx.x & 31;
     const int raw = e > s ? (int)min(e - s, 0x7fffffffu) : 0;
     const int use = raw < maxlen ? raw : maxlen;
@@ -246,41 +274,32 @@ __device__ void decode_record_warp(const unsigned char* __restrict__ text, u32 s
     }
     if (lane == 0) *len_out = (u32)n;
     __syncwarp();
+    return n;
 }
 
-// redo the flagged records (all of them when reverse != 0), then accumulate "kmer(s) in reads" / reads kept
+// Redo the records on the redo list (every record when reverse != 0), one warp per record, and replace what k_decode_fast counted for
+// each of them by what it really holds.  A small fixed grid: on clean text the list is empty and every warp leaves at once.
 __global__ void __launch_bounds__(256) k_decode_fix(const unsigned char* __restrict__ text, const u32* __restrict__ seq_start, const u32* __restrict__ seq_end,
                                                     u64 n_rec, int maxlen, int reverse, int K, int W64, u64* __restrict__ words, u32* __restrict__ lens,
-                                                    const u8* __restrict__ bad, u64* counters) {
+                                                    const u32* __restrict__ redo, const u32* __restrict__ n_redo, u64* counters) {
     const int lane = threadIdx.x & 31;
     const u64 warp0 = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((u64)gridDim.x * blockDim.x) >> 5;
-    u64 inst = 0, kept = 0;
-    for (u64 r0 = warp0 * 32; r0 < n_rec; r0 += nwarps * 32) {
-        const u64 r = r0 + lane;
-        const bool flag = r < n_rec && (reverse || bad[r]);
-        unsigned todo = __ballot_sync(0xffffffffu, flag);
-        while (todo) {
-            const int l = __ffs(todo) - 1;
-            todo &= todo - 1;
-            const u64 rr = r0 + l;
-            decode_record_warp(text, seq_start[rr], seq_end[rr], maxlen, reverse, W64, words + rr * (u64)W64, lens + rr);
-        }
-        if (r < n_rec) {
-            const int n = (int)lens[r];
-            if (n >= K + 1) { inst += (u64)(n - K + 1); kept++; }   // reads shorter than K+1 are skipped (prlHashReads.c:504,642)
+    const u64 n = reverse ? n_rec : (u64)*n_redo;
+    if (n == 0) return;   // grid-uniform
+    if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd((unsigned long long*)&counters[C_REDO], (unsigned long long)n);
+    u64 inst = 0, kept = 0;   // deltas, modulo 2^64
+    for (u64 i = warp0; i < n; i += nwarps) {
+        const u64 rr = reverse ? i : (u64)redo[i];
+        const int before = (int)lens[rr];
+        __syncwarp();
+        const int after = decode_record_warp(text, seq_start[rr], seq_end[rr], maxlen, reverse, W64, words + rr * (u64)W64, lens + rr);
+        if (lane == 0) {
+            inst += read_instances(after, K) - read_instances(before, K);
+            kept += (u64)(read_instances(after, K) ? 1 : 0) - (u64)(read_instances(before, K) ? 1 : 0);
         }
     }
-    __shared__ u64 s_inst, s_kept;
-    if (threadIdx.x == 0) { s_inst = 0; s_kept = 0; }
-    __syncthreads();
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        inst += __shfl_down_sync(0xffffffffu, inst, d);
-        kept += __shfl_down_sync(0xffffffffu, kept, d);
-    }
-    if (lane == 0 && (inst | kept)) { atomicAdd(&s_inst, inst); atomicAdd(&s_kept, kept); }
-    __syncthreads();
-    if (threadIdx.x == 0 && (s_inst | s_kept)) { atomicAdd(&counters[C_INSTANCES], s_inst); atomicAdd(&counters[C_KEPT], s_kept); }
+    cta_add_u64(inst, &counters[C_INSTANCES]);
+    cta_add_u64(kept, &counters[C_KEPT]);
 }
 
 // ------------------------------------------------------------------------------------------------ the decode of one text chunk
@@ -311,16 +330,18 @@ DecodeLines decode_lines(const unsigned char* d_text, size_t nbytes, int fastq, 
     const u64 n_lines = h_cnt[C_MISC0];
     // a final line without '\n' still counts (the reference's FASTQ path tolerates it; its FASTA path does not)
     const bool open_tail = *h_last != '\n';
-    DecodeLines L{nullptr, nullptr, nullptr, (n_lines + (open_tail ? 1 : 0)) / lpr};
+    DecodeLines L{nullptr, nullptr, nullptr, nullptr, nullptr, (n_lines + (open_tail ? 1 : 0)) / lpr};
     if ((n_lines + (open_tail ? 1 : 0)) % lpr != 0)
         throw std::runtime_error("pgb200: text chunk does not hold whole FASTA/FASTQ records (line count not a multiple of 2/4)");
     const u64 n_rec = L.n_rec;
     if (n_rec == 0) return L;
-    line_buf.ensure(2 * n_rec * sizeof(u32) + n_rec + 256);
+    line_buf.ensure((4 * n_rec + 1) * sizeof(u32) + 256);
     L.seq_start = line_buf.template as<u32>();
     L.seq_end = L.seq_start + n_rec;
-    L.bad = reinterpret_cast<u8*>(L.seq_end + n_rec);
-    PG_CUDA(cudaMemsetAsync(L.bad, 0, n_rec, sd));
+    L.n_redo = L.seq_end + n_rec;
+    L.flag = L.n_redo + 1;
+    L.redo = L.flag + n_rec;
+    PG_CUDA(cudaMemsetAsync(L.n_redo, 0, (n_rec + 1) * sizeof(u32), sd));   // the count and the flags
     if (open_tail) PG_CUDA(cudaMemsetAsync(L.seq_end, 0, n_rec * sizeof(u32), sd));   // FASTQ: the open line is the quality line
     k_line_index<<<nl_blocks, 256, 0, sd>>>(t16, (u64)nbytes, n_tiles, tile_base, lshift, n_rec, L.seq_start, L.seq_end, d_cnt);
     PG_CUDA(cudaGetLastError());
@@ -335,12 +356,11 @@ DecodeLines decode_lines(const unsigned char* d_text, size_t nbytes, int fastq, 
 void decode_records(const unsigned char* d_text, size_t nbytes, const DecodeLines& L, int maxlen, int reverse, int K, int W64, int n_sm, u64* words,
                     u32* lens, u64* d_cnt, cudaStream_t sd) {
     const u64 n_rec = L.n_rec, total = n_rec * (u64)W64;
-    k_decode_fast<<<(unsigned)std::min<u64>((total + 255) / 256, (u64)n_sm * 64), 256, 0, sd>>>(d_text, (u64)nbytes, L.seq_start, L.seq_end, n_rec, maxlen, W64,
-                                                                                            words, lens, L.bad);
+    k_decode_fast<<<(unsigned)std::min<u64>((total + 255) / 256, (u64)n_sm * 64), 256, 0, sd>>>(d_text, (u64)nbytes, L.seq_start, L.seq_end, n_rec, maxlen, K,
+                                                                                            W64, words, lens, L.flag, L.redo, L.n_redo, d_cnt);
     PG_CUDA(cudaGetLastError());
-    const u64 fix_warps = (n_rec + 31) / 32;
-    k_decode_fix<<<(unsigned)std::min<u64>((fix_warps + 7) / 8, (u64)n_sm * 32), 256, 0, sd>>>(d_text, L.seq_start, L.seq_end, n_rec, maxlen, reverse, K, W64,
-                                                                                         words, lens, L.bad, d_cnt);
+    k_decode_fix<<<(unsigned)std::min<u64>((n_rec + 7) / 8, (u64)n_sm * 8), 256, 0, sd>>>(d_text, L.seq_start, L.seq_end, n_rec, maxlen, reverse, K, W64,
+                                                                                    words, lens, L.redo, L.n_redo, d_cnt);
     PG_CUDA(cudaGetLastError());
 }
 

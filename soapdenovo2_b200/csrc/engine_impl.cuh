@@ -72,7 +72,8 @@ struct ReadChunk {
 };
 
 enum Counter { C_DISTINCT = 0, C_INSTANCES, C_KEPT, C_LINEAR, C_REMOVED, C_MISC0, C_MISC1, C_MISC2, C_BADFMT, C_XERR, C_XUSED, C_RESERVED, C_DEFER, C_MAXU,
-               C_XSEGS, C_XEPOCH, C_SPILLKEYS, C_COUNT };   // C_SPILLKEYS: keys the aggregation stored WITHOUT the fused sweeps
+               C_XSEGS, C_XEPOCH, C_SPILLKEYS, C_REDO, C_COUNT };   // C_SPILLKEYS: keys the aggregation stored WITHOUT the fused sweeps;
+                                                                 // C_REDO: records decoded by the general rules (k_decode_fix)
 
 // What an aggregation launch reports: C_XERR .. C_MAXU, read with one copy
 struct FlushOutcome { u64 xerr, xused, reserved, defer, maxu; };
@@ -101,7 +102,9 @@ enum class PassSweeps { Untouched, Fused, Plain };
 struct DecodeLines {
     u32* seq_start;
     u32* seq_end;
-    u8* bad;
+    u32* n_redo;   // records the fast decode could not handle (general rules: k_decode_fix) ...
+    u32* redo;     // ... and their indices
+    u32* flag;     // [n_rec] 1 once a record is on the redo list
     u64 n_rec;
 };
 void check_format(const u64* h_cnt);   // throws the malformed-input error when the line index flagged a bad record
@@ -191,10 +194,10 @@ public:
     SkmGeom skm_geom_;
     u32 skm_own_lo_ = 0, skm_own_hi_ = 0;
     int skm_own_shift_ = -1;
+    int skm_part_threads_ = 128;
     DevBuf skm_cnt_, skm_segoff_, skm_cursor_, skm_scan_, skm_side_;
     DevBuf skm_scratch_;               // SkmScratch (skm.cu): the exchange's device-side cursors, scan total and segment list
     DevBuf skm_deferred_[2];           // deferred buckets of an aggregation launch, read by the re-run that writes the other list
-    int skm_part_threads_ = 128;
     // the exchange arena: [SKM_ARENA_HALVES][nseg | ring | offsets | world x cap_pair records]; xa_peer_[o] = owner o's arena as mapped here
     SkmArenaGeom xa_geom_;
     DevBuf xa_buf_;

@@ -213,6 +213,9 @@ void EngineT<NW>::finish_pass1(Pass1Stats* st) {
     p1_.distinct = h_cnt_[C_DISTINCT];
     p1_.table_slots = cap_;
     n_nodes_ = p1_.distinct;
+    if (prm_.verbose)
+        fprintf(stderr, "[pgb200] pass 1: %llu records, %llu of them decoded by the general rules\n", (unsigned long long)total_records_,
+                (unsigned long long)h_cnt_[C_REDO]);
     if (st) *st = p1_;
 }
 

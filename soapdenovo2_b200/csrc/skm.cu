@@ -6,8 +6,8 @@
 //                      device_scan    bucket counts -> offsets of the chunk's bucket-major record blob
 //                      k_skm_publish  reserves room for the blob in every owner's arena (sender-private region: no coordination),
 //                                     writes the segment descriptor and the owner's slice of the offsets INTO THE OWNER'S MEMORY
-//                      k_skm_scatter  builds the self-contained records and stores each one at its final position in its owner's
-//                                     arena: plain stores for the local GPU, NVLink peer stores (CUDA IPC / peer access mappings)
+//                      k_skm_scatter  one lane per run: builds the self-contained records and stores each one at its final position
+//                                     in its owner's arena: plain stores for the local GPU, NVLink peer stores (CUDA IPC / peer access mappings)
 //                                     for the others.  Partition and "all-to-all" are the same kernel; no library collective, no
 //                                     staging buffer, no second pass over the records.
 //   flush (end of pass 1 / arena full):  k_skm_apply over the owned buckets; buckets whose worst case does not fit the global table
@@ -55,6 +55,8 @@ struct CountEmit {
     }
 };
 
+// One thread per read.  (The warp routine of k_skm_rescan, skm_warp_scan_read, makes the same runs but issues about three times the
+// instructions per read at 150 bases: 27.6 against 9.6 ms per step on H100, DESIGN.md §5.)
 __global__ void __launch_bounds__(SKM_PART_THREADS) k_skm_count(SkmGeom g, const u64* __restrict__ words, const u32* __restrict__ lens, u64 n_rec, int W64,
                                                                u32* cnt, u32* side, u8* nruns) {
     extern __shared__ u32 s_ring[];   // [g.w][blockDim.x]: one column per thread, bank = thread -> conflict-free
@@ -179,28 +181,30 @@ __device__ __forceinline__ void skm_emit_rec(const SkmSendArgs& a, u32* cursor_b
     skm_store_rec<NW>(a.peer_recs[o] + idx * (NW + 2), r);
 }
 
-// one thread per read: the runs come from the side buffer (no minimizer work), the records go to their owners
+// one lane per run: a warp takes two reads, a half-warp per read and one side-row entry per lane, so the side rows load coalesced and
+// every run of the warp has its cursor atomic and its record store in flight at once.  A run starts where the runs before it in its
+// row end (prefix over the half-warp).  The runs come from the side buffer: no minimizer work here.
 template <int NW>
 __global__ void __launch_bounds__(256) k_skm_scatter(SkmSendArgs a, int K, const u64* __restrict__ words, u64 n_rec, int W64, u64 ord_base, u64 ord_stride,
                                                      const u32* __restrict__ side, const u8* __restrict__ nruns, u32* cursor_b) {
-    for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < n_rec; r += (u64)gridDim.x * blockDim.x) {
-        const int nr = nruns[r];
-        if (nr == 255 || nr == 0) continue;
-        const u64* wp = words + r * (u64)W64;
-        const u64 ordinal = ord_base + r * ord_stride;
-        const uint4* row = reinterpret_cast<const uint4*>(side + r * SKM_SIDE_RUNS);
-        int start = 0;
-        for (int q = 0; q < nr; q += 4) {
-            const uint4 v = __ldg(row + (q >> 2));
-            const u32 e[4] = {v.x, v.y, v.z, v.w};
+    static_assert(SKM_SIDE_RUNS == 16, "a half-warp holds one side row");
+    const int lane = threadIdx.x & 31, slot = lane & 15;
+    const u64 n_pairs = (n_rec + 1) / 2;
+    const u64 warp0 = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((u64)gridDim.x * blockDim.x) >> 5;
+    for (u64 p = warp0; p < n_pairs; p += nwarps) {
+        const u64 r = 2 * p + (lane >> 4);
+        int nr = r < n_rec ? (int)nruns[r] : 0;
+        if (nr == 255) nr = 0;   // more runs than the side row holds: k_skm_rescan
+        const bool act = slot < nr;
+        const u32 e = act ? __ldg(side + r * SKM_SIDE_RUNS + slot) : 0u;
+        const int n = act ? skm_side_n(e) : 0;
+        int inc = n;
 #pragma unroll
-            for (int x = 0; x < 4; x++) {
-                if (q + x >= nr) break;
-                const int n = skm_side_n(e[x]);
-                skm_emit_rec<NW>(a, cursor_b, K, wp, W64, ordinal, skm_side_bucket(e[x]), start, n, skm_side_last(e[x]));
-                start += n;
-            }
+        for (int d = 1; d < 16; d <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, inc, d, 16);
+            if (slot >= d) inc += v;
         }
+        if (act) skm_emit_rec<NW>(a, cursor_b, K, words + r * (u64)W64, W64, ord_base + r * ord_stride, skm_side_bucket(e), inc - n, n, skm_side_last(e));
     }
 }
 
@@ -213,17 +217,24 @@ struct RescanEmit {
     const u64* wp;
     int W64;
     u64 ordinal;
-    __device__ __forceinline__ void operator()(u32 b, int s, int n, bool last) { skm_emit_rec<NW>(a, cursor_b, K, wp, W64, ordinal, b, s, n, last); }
+    __device__ __forceinline__ void operator()(u32 b, int s, int n, bool last, int) const { skm_emit_rec<NW>(a, cursor_b, K, wp, W64, ordinal, b, s, n, last); }
 };
+// the lanes of a warp check 32 reads at a time; the warp re-scans each flagged one (skm_warp_scan_read)
 template <int NW>
 __global__ void __launch_bounds__(SKM_PART_THREADS) k_skm_rescan(SkmSendArgs a, SkmGeom g, const u64* __restrict__ words, const u32* __restrict__ lens, u64 n_rec,
                                                                 int W64, u64 ord_base, u64 ord_stride, const u8* __restrict__ nruns, u32* cursor_b) {
-    extern __shared__ u32 s_ring[];
-    for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < n_rec; r += (u64)gridDim.x * blockDim.x) {
-        if (nruns[r] != 255) continue;
-        const u64* wp = words + r * (u64)W64;
-        RescanEmit<NW> e{a, cursor_b, g.K, wp, W64, ord_base + r * ord_stride};
-        skm_scan_read(g, wp, (int)lens[r], s_ring + threadIdx.x, (int)blockDim.x, e);
+    __shared__ u32 s_ring[SKM_PART_THREADS / 32][SKM_WARP_RING];
+    const int lane = threadIdx.x & 31;
+    const u64 warp0 = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((u64)gridDim.x * blockDim.x) >> 5;
+    for (u64 r0 = warp0 * 32; r0 < n_rec; r0 += nwarps * 32) {
+        unsigned todo = __ballot_sync(0xffffffffu, r0 + lane < n_rec && nruns[r0 + lane] == 255);
+        while (todo) {
+            const u64 r = r0 + (__ffs(todo) - 1);
+            todo &= todo - 1;
+            const u64* wp = words + r * (u64)W64;
+            const RescanEmit<NW> e{a, cursor_b, g.K, wp, W64, ord_base + r * ord_stride};
+            skm_warp_scan_read(g, wp, W64, (int)lens[r], s_ring[threadIdx.x >> 5], e);
+        }
     }
 }
 
@@ -692,13 +703,11 @@ void EngineT<NW>::skm_init() {
     skm_scratch_.alloc(sizeof(SkmScratch));
     PG_CUDA(cudaMemsetAsync(skm_scratch_.p, 0, sizeof(SkmScratch), st_));
     for (DevBuf& d : skm_deferred_) d.alloc((size_t)(skm_own_hi_ - skm_own_lo_ + 1) * sizeof(u32));
+    if (skm_geom_.w > SKM_RING_TILES * 32 - 63) throw std::runtime_error("pgb200: minimizer window too long for the partition kernels");
     skm_part_threads_ = SKM_PART_THREADS;
     while ((size_t)skm_part_threads_ * skm_geom_.w * sizeof(u32) > 160 * 1024 && skm_part_threads_ > 32) skm_part_threads_ /= 2;
     const size_t ring = (size_t)skm_part_threads_ * skm_geom_.w * sizeof(u32);
-    if (ring > 48 * 1024) {
-        PG_CUDA(cudaFuncSetAttribute(k_skm_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
-        PG_CUDA(cudaFuncSetAttribute(k_skm_rescan<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
-    }
+    if (ring > 48 * 1024) PG_CUDA(cudaFuncSetAttribute(k_skm_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
     PG_CUDA(cudaFuncSetAttribute(k_skm_apply<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)skm_apply_smem<NW>()));
     if (prm_.verbose) fprintf(stderr, "[pgb200] aggregated pass 1: %u buckets (%u owned by GPU %d of %d), minimizer length %d, window %d\n", skm_geom_.n_buckets,
                               skm_own_hi_ - skm_own_lo_, prm_.rank, world, skm_geom_.m, skm_geom_.w);
@@ -878,12 +887,12 @@ void EngineT<NW>::skm_feed_chunk(size_t ci) {
     const int world = xa_geom_.world;
     PG_CUDA(cudaMemsetAsync(skm_cnt_.p, 0, (B + 1) * sizeof(u32), st_));
     PG_CUDA(cudaMemsetAsync(skm_cursor_.p, 0, (B + 1) * sizeof(u32), st_));
-    const size_t ring = (size_t)skm_part_threads_ * skm_geom_.w * sizeof(u32);
-    const unsigned blocks = (unsigned)std::min<u64>((ch.n_rec + skm_part_threads_ - 1) / skm_part_threads_, (u64)n_sm_ * 16);
+    constexpr int part_warps = SKM_PART_THREADS / 32;
     skm_side_.ensure(ch.n_rec * (SKM_SIDE_RUNS * sizeof(u32) + 1) + 256);
     u32* side = skm_side_.template as<u32>();
     u8* nruns = reinterpret_cast<u8*>(side + ch.n_rec * SKM_SIDE_RUNS);
-    k_skm_count<<<blocks, skm_part_threads_, ring, st_>>>(skm_geom_, ch.words, ch.len, ch.n_rec, W64_, skm_cnt_.template as<u32>(), side, nruns);
+    const size_t ring = (size_t)skm_part_threads_ * skm_geom_.w * sizeof(u32);
+    k_skm_count<<<(unsigned)std::min<u64>((ch.n_rec + skm_part_threads_ - 1) / skm_part_threads_, (u64)n_sm_ * 16), skm_part_threads_, ring, st_>>>(skm_geom_, ch.words, ch.len, ch.n_rec, W64_, skm_cnt_.template as<u32>(), side, nruns);
     PG_CUDA(cudaGetLastError());
     device_scan(BucketCntIn{skm_cnt_.template as<u32>()}, BucketOffOut{skm_segoff_.template as<u32>()}, (u64)B, skm_scan_.template as<u64>(),
                 &skm_scratch_.template as<SkmScratch>()->blob_total, st_);
@@ -892,9 +901,9 @@ void EngineT<NW>::skm_feed_chunk(size_t ci) {
     k_skm_publish<<<(unsigned)std::min<u64>(((u64)B + world + 255) / 256, (u64)n_sm_ * 8), 256, 0, st_>>>(a);
     PG_CUDA(cudaGetLastError());
     u32* cursor_b = skm_cursor_.template as<u32>();
-    k_skm_scatter<NW><<<(unsigned)std::min<u64>((ch.n_rec + 255) / 256, (u64)n_sm_ * 16), 256, 0, st_>>>(a, prm_.K, ch.words, ch.n_rec, W64_, ch.ord_base, ch.ord_stride, side, nruns, cursor_b);
+    k_skm_scatter<NW><<<(unsigned)std::min<u64>((ch.n_rec + 15) / 16, (u64)n_sm_ * 16), 256, 0, st_>>>(a, prm_.K, ch.words, ch.n_rec, W64_, ch.ord_base, ch.ord_stride, side, nruns, cursor_b);
     PG_CUDA(cudaGetLastError());
-    k_skm_rescan<NW><<<blocks, skm_part_threads_, ring, st_>>>(a, skm_geom_, ch.words, ch.len, ch.n_rec, W64_, ch.ord_base, ch.ord_stride, nruns, cursor_b);
+    k_skm_rescan<NW><<<(unsigned)std::min<u64>((ch.n_rec + 32 * part_warps - 1) / (32 * part_warps), (u64)n_sm_ * 16), SKM_PART_THREADS, 0, st_>>>(a, skm_geom_, ch.words, ch.len, ch.n_rec, W64_, ch.ord_base, ch.ord_stride, nruns, cursor_b);
     PG_CUDA(cudaGetLastError());
     if (xa_reads_cum_.empty()) xa_reads_cum_.push_back(0);
     xa_reads_cum_.push_back(xa_reads_cum_.back() + ch.n_rec);

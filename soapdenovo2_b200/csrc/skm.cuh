@@ -146,6 +146,107 @@ PG_HD void skm_scan_read(const SkmGeom& g, const u64* wp, int L, u32* scratch, i
     if (run_len) emit(cur_b, run_start, run_len, true);
 }
 
+#if defined(__CUDACC__)
+// The same runs as skm_scan_read, computed by one warp per read (the partition kernels of skm.cu; tests/host_skm_warp.cu checks it
+// against skm_scan_read).  The lanes take 32 consecutive positions at a time:
+//   * m-mer tile T = positions 32T .. 32T+31.  Lane l builds its m-mer straight from the packed words (bases 32T+l .. are bits 2l ..
+//     of words T, T+1): the reverse complement is those 2m bits XOR 0b10.., the forward m-mer their 2-bit groups reversed.  The tile's
+//     order values and their prefix and suffix minima go to a per-warp ring of SKM_RING_TILES tiles in shared memory.
+//   * k-mer tile t = k-mers 32t .. 32t+31; k-mer j needs the minimum over m-mer positions j .. e = j+w-1.  A window that crosses a
+//     tile boundary is suffix(tile of j) + whole tiles between + prefix(tile of e); a window inside one tile (only when w <= 32) is
+//     a sparse-table query over the tile (two overlapping power-of-two ranges).  Nothing is kept per thread, and the footprint does
+//     not grow with w: a window spans at most ceil((31 + w) / 32) + 1 <= 5 tiles for w <= 113 (K <= 127).
+//   * runs: a cut wherever the bucket changes (ballot), and every SKM_MAX_RUN k-mers since the last change, carried across tiles; the
+//     lanes that start a run know its length once the next start is known, so the run that is still open at the end of a tile is
+//     carried and emitted by the tile that holds the next start (or at the end of the read, with `last`).
+// emit(bucket, first k-mer position, count, last, run index) is called once per run, by one lane, runs of one tile concurrently.
+// Returns the number of runs (warp-uniform).  `ring` holds SKM_WARP_RING words for this warp.
+constexpr int SKM_RING_TILES = 8;
+constexpr int SKM_WARP_RING = 3 * SKM_RING_TILES * 32;
+static_assert(SKM_MAX_RUN == 32, "forced cuts are counted modulo the tile width");
+template <class Emit>
+__device__ __forceinline__ int skm_warp_scan_read(const SkmGeom& g, const u64* wp, int W64, int L, u32* ring, Emit& emit) {
+    const int K = g.K, m = g.m, w = g.w;
+    if (L < K + 1) return 0;   // reads shorter than K+1 contribute nothing (prlHashReads.c:504,642)
+    const unsigned full = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const unsigned lane_lt = (1u << lane) - 1u, lane_le = lane_lt | (1u << lane);
+    const int nk = L - K + 1, nq = L - m + 1;   // k-mers, m-mer positions
+    const int D = (31 + w - 1) >> 5;           // m-mer tiles ahead of the k-mer tile that its windows reach
+    u32* const raw = ring;
+    u32* const pre = ring + SKM_RING_TILES * 32;
+    u32* const suf = pre + SKM_RING_TILES * 32;
+    const u32 cmask = 0xAAAAAAAAu & g.mmask;
+    auto slot = [](int T) { return (T & (SKM_RING_TILES - 1)) * 32; };
+    auto fill = [&](int T) {
+        if (32 * T >= nq) return;   // warp-uniform
+        const u64 w0 = wp[T], w1 = T + 1 < W64 ? wp[T + 1] : 0ull;
+        const int sh = 2 * lane;
+        const u32 x = (u32)(sh ? (w0 >> sh) | (w1 << (64 - sh)) : w0) & g.mmask;
+        u32 y = __brev(x);
+        y = ((y >> 1) & 0x55555555u) | ((y << 1) & 0xAAAAAAAAu);
+        const u32 ov = 32 * T + lane < nq ? skm_order(y >> (32 - 2 * m), x ^ cmask) : 0xFFFFFFFFu;
+        u32 p = ov, s = ov;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const u32 u = __shfl_up_sync(full, p, d), v = __shfl_down_sync(full, s, d);
+            if (lane >= d) p = min(p, u);
+            if (lane + d < 32) s = min(s, v);
+        }
+        raw[slot(T) + lane] = ov;
+        pre[slot(T) + lane] = p;
+        suf[slot(T) + lane] = s;
+    };
+    int len2 = 1;                               // largest power of two <= w
+    while (2 * len2 <= w) len2 *= 2;
+    for (int T = 0; T < D; T++) fill(T);
+    u32 carry_b = 0, open_b = 0;
+    int carry_seg = 0, open_start = 0, open_idx = 0, nrun = 0;
+    for (int t = 0; 32 * t < nk; t++) {
+        __syncwarp();
+        fill(t + D);
+        __syncwarp();
+        const int j = 32 * t + lane;
+        const bool valid = j < nk;
+        const int e = j + w - 1, Te = e >> 5, le = e & 31;
+        u32 mv = min(suf[slot(t) + lane], pre[slot(Te) + le]);
+        for (int T = t + 1; T < Te; T++) mv = min(mv, pre[slot(T) + 31]);
+        if (w <= 32) {                          // warp-uniform
+            u32 sp = raw[slot(t) + lane];       // -> min over lane .. lane+len2-1 (cut at the tile end)
+            for (int d = 1; d < len2; d <<= 1) {
+                const u32 u = __shfl_down_sync(full, sp, d);
+                if (lane + d < 32) sp = min(sp, u);
+            }
+            const u32 u = __shfl_sync(full, sp, (le - len2 + 1) & 31);
+            if (Te == t) mv = min(sp, u);
+        }
+        const u32 b = skm_bucket(mv, g.n_buckets);
+        u32 bprev = __shfl_up_sync(full, b, 1);
+        if (lane == 0) bprev = carry_b;
+        const unsigned chg = __ballot_sync(full, valid && (j == 0 || b != bprev));
+        const unsigned below = chg & lane_le;
+        const int seg = below ? 32 * t + 31 - __clz(below) : carry_seg;   // first k-mer of this lane's bucket stretch
+        const bool st = valid && ((j - seg) & (SKM_MAX_RUN - 1)) == 0;
+        const unsigned stm = __ballot_sync(full, st);
+        if (stm) {
+            if (nrun && lane == 0) emit(open_b, open_start, 32 * t + __ffs(stm) - 1 - open_start, false, open_idx);
+            const unsigned after = stm & ~lane_le;
+            if (st && after) emit(b, j, __ffs(after) - 1 - lane, false, nrun + __popc(stm & lane_lt));
+            const int hs = 31 - __clz(stm);     // the tile's last run stays open
+            open_b = __shfl_sync(full, b, hs);
+            open_start = 32 * t + hs;
+            open_idx = nrun + __popc(stm) - 1;
+            nrun += __popc(stm);
+        }
+        carry_b = __shfl_sync(full, b, 31);
+        if (chg) carry_seg = 32 * t + 31 - __clz(chg);
+    }
+    if (lane == 0) emit(open_b, open_start, nk - open_start, true, open_idx);
+    __syncwarp();
+    return nrun;
+}
+#endif
+
 // bucket of ONE k-mer given as a Kmer (used by tests: every instance of a canonical k-mer must map to the same bucket)
 template <int NW>
 PG_HD u32 skm_bucket_of_kmer(const SkmGeom& g, const Kmer<NW>& k) {
