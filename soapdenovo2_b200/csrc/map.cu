@@ -19,16 +19,25 @@
 // first occurrence (later members are cleared as they are counted), `counter2` / `counter` / the strict `>` that gives a tie to the
 // earlier group.  Per-read state is a handful of registers whatever the read length, so no read spills; the span lives in global
 // memory (8 B per k-mer, at most 100 M k-mers per batch, the reference's buffer_size).
+//
+// Long reads (prlLongRead2Ctg, prlRead2Ctg.c:1080-1298).  A batch holds 100 M / (longReadLen - K + 1) reads -- 20 000 at a 5 kbp
+// cutoff -- so one thread per read would leave most of the GPU idle, each thread doing thousands of dependent lookups.  k_map_long
+// gives each read one CTA: the threads take contiguous slices of at least MAP_SEG k-mers, build the slice's first forward / reverse-
+// complement pair and roll from there, look each k-mer up with map_lookup and write the hit to the span as k_map_reads does.  Each
+// hit is also counted in a shared-memory group table keyed by contig id; parse1read's result is a function of the groups' (count,
+// first index) alone, and the table stays exact past its size by grouping the leftover ids in further rounds (map_group.cuh has
+// the argument).  The reads are stored at their own packed length, located by word offsets.
 #include "engine_impl.cuh"
 #include "map.h"
+#include "map_group.cuh"
 #include <algorithm>
+#include <cstdlib>
 
 #pragma GCC visibility push(hidden)
 namespace pgb {
 
-constexpr u64 HIT_VALID = 1ull << 63;
-constexpr int HIT_SMALLER_SHIFT = 58;
-constexpr int MAP_SEG = 64;   // contig k-mers per thread of k_map_contigs
+constexpr int MAP_SEG = 64;   // contig k-mers per thread of k_map_contigs; the least k-mers per thread of k_map_long
+constexpr int MAP_LONG_THREADS = 128;
 
 struct CtgSeg {
     u64 base;      // global base index of the segment's first k-mer
@@ -172,6 +181,85 @@ __global__ void __launch_bounds__(128) k_map_reads(Table<NW> t, KParams<NW> kp, 
     }
 }
 
+// one CTA per read (grid-stride over the batch); read r is words[wofs[r] ...], its hits go to hits[kofs[r] ...]
+template <int NW>
+__global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KParams<NW> kp, const u64* __restrict__ words, const u64* __restrict__ wofs,
+                                                               const u32* __restrict__ lens, const u64* __restrict__ kofs, u64 n_reads, int alignlen,
+                                                               u32 n_groups, u64* __restrict__ hits, MapHit* __restrict__ out) {
+    __shared__ u32 s_id[MAP_GROUPS], s_cnt[MAP_GROUPS], s_first[MAP_GROUPS];
+    __shared__ GroupAcc s_acc;
+    __shared__ int s_pending;
+    const int K = kp.K, tid = threadIdx.x, nthr = blockDim.x;
+    const GroupTab g{s_id, s_cnt, s_first, n_groups};
+    for (u64 r = blockIdx.x; r < n_reads; r += gridDim.x) {
+        const int len = (int)lens[r];
+        const u64* w = words + wofs[r];
+        u64* h = hits + kofs[r];
+        const u32 nk = len >= K + 1 ? (u32)(len - K + 1) : 0u;   // chopKmer4read returns early below K+1 (the span is empty)
+        group_clear(g, tid, nthr);
+        if (tid == 0) { s_acc = GroupAcc{0u, 0u, 0ull}; s_pending = 0; }
+        __syncthreads();
+        // this thread's slice: [j0, j1), at least MAP_SEG k-mers unless the read has fewer
+        const u32 per = max((u32)MAP_SEG, (nk + nthr - 1) / nthr);
+        const u32 j0 = min(nk, (u32)tid * per), j1 = min(nk, j0 + per);
+        if (j0 < j1) {
+            const KPair<NW> k0 = first_kmer(w, j0, kp);
+            Kmer<NW> f = k0.f, rc = k0.rc;
+            for (u32 j = j0; j < j1; j++) {
+                if (j > j0) {
+                    const u32 p = j + K - 1;
+                    const unsigned c = (unsigned)(w[p >> 5] >> (2 * (p & 31))) & 3u;
+                    f = knext(f, c, kp);
+                    rc = kprev_reg(rc, c ^ 2u, kp);
+                }
+                const bool smaller = kless(f, rc);
+                const u64 v = map_lookup(t, kcanon(f, rc, smaller));
+                h[j] = v ? v | ((u64)smaller << HIT_SMALLER_SHIFT) : 0ull;
+                if (v) group_add_hit(h, j, g, &s_pending);
+            }
+        }
+        // parse1read: fold the groups; ids left over when the table is full are grouped in further rounds
+        const int alldgn = len > alignlen ? alignlen : len;
+        const u32 multi = (u32)(alldgn - K + 1 < 2 ? 2 : alldgn - K + 1);
+        for (;;) {
+            __syncthreads();
+            group_fold(g, K, multi, tid, nthr, &s_acc);
+            const int more = s_pending;   // no thread writes it between the barriers around this read
+            __syncthreads();
+            if (!more) break;
+            group_clear(g, tid, nthr);
+            if (tid == 0) s_pending = 0;
+            __syncthreads();
+            group_round(h, nk, g, tid, nthr, &s_pending);
+        }
+        if (tid == 0) {
+            const GroupAcc a = s_acc;
+            MapHit o{0u, 0, 0, 0u};
+            if (a.counter) {
+                const u32 bj = group_best_j(a);
+                const u64 best = h[bj];
+                const unsigned twin = (unsigned)(best >> 56) & 3u, smaller = (unsigned)(best >> HIT_SMALLER_SHIFT) & 1u;
+                o.ctg = (u32)best;
+                o.node_pos = (int)((best >> 32) & 0xFFFFFFu);
+                o.i = (int)bj + 1;
+                o.flags = MAP_PLACED | (twin == smaller ? MAP_MINUS : 0u) | (a.counter2 > 1 ? MAP_FOOTPRINT : 0u);
+            }
+            out[r] = o;
+        }
+        __syncthreads();   // s_acc is read before the next read resets it
+    }
+}
+
+// strided decode output (stride words per read) -> packed at each read's own length, read r at ofs[r]
+__global__ void __launch_bounds__(256) k_pack_reads(const u64* __restrict__ in, int stride, const u32* __restrict__ lens, const u64* __restrict__ ofs,
+                                                    u64 n, u64* __restrict__ packed) {
+    const int lane = threadIdx.x & 31;
+    for (u64 r = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += ((u64)gridDim.x * blockDim.x) >> 5) {
+        const u32 nw = (lens[r] + 31) / 32;
+        for (u32 i = lane; i < nw; i += 32) packed[ofs[r] + i] = in[r * (u64)stride + i];
+    }
+}
+
 template <int NW>
 class MapEngineT : public IMapEngine {
 public:
@@ -221,7 +309,8 @@ public:
         *distinct = h_cnt_[C_DISTINCT];
     }
 
-    void decode_text(const char* text, size_t nbytes, int fastq, int reverse, int maxlen, std::vector<u64>* words, std::vector<u32>* lens) override {
+    void decode_text(const char* text, size_t nbytes, int fastq, int reverse, int maxlen, int stride, std::vector<u64>* words,
+                     std::vector<u32>* lens) override {
         if (nbytes == 0) return;
         if (nbytes >= (1ull << 32)) throw std::runtime_error("pgb200: a text chunk must be smaller than 4 GiB (feed it in pieces)");
         PG_CUDA(cudaSetDevice(device_));
@@ -232,17 +321,35 @@ public:
         const DecodeLines L = decode_lines(d_text, nbytes, fastq, n_sm_, scan_buf_, line_buf_, cnt_.as<u64>(), h_cnt_, st_);
         if (L.n_rec == 0) return;
         const u64 n = L.n_rec;
-        read_words_.ensure(n * W64_ * sizeof(u64));
+        const int S = stride > 0 ? stride : std::max(1, (maxlen + 31) / 32);   // the decode's stride: room for maxlen bases
+        read_words_.ensure(n * S * sizeof(u64));
         read_lens_.ensure(n * sizeof(u32));
-        decode_records(d_text, nbytes, L, maxlen, reverse, K_, W64_, n_sm_, read_words_.as<u64>(), read_lens_.as<u32>(), cnt_.as<u64>(), st_);
-        PG_CUDA(cudaEventRecord(ev_[1], st_));
+        decode_records(d_text, nbytes, L, maxlen, reverse, K_, S, n_sm_, read_words_.as<u64>(), read_lens_.as<u32>(), cnt_.as<u64>(), st_);
+        if (stride > 0) PG_CUDA(cudaEventRecord(ev_[1], st_));
         const size_t w0 = words->size(), l0 = lens->size();
-        words->resize(w0 + n * W64_);
         lens->resize(l0 + n);
-        PG_CUDA(cudaMemcpyAsync(words->data() + w0, read_words_.p, n * W64_ * sizeof(u64), cudaMemcpyDeviceToHost, st_));
         PG_CUDA(cudaMemcpyAsync(lens->data() + l0, read_lens_.p, n * sizeof(u32), cudaMemcpyDeviceToHost, st_));
         // the line index of THIS chunk flags malformed records (decode_lines checked the counters before it ran)
         PG_CUDA(cudaMemcpyAsync(h_cnt_, cnt_.p, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st_));
+        u64 n_words = n * S;
+        const u64* src = read_words_.as<u64>();
+        if (stride <= 0) {   // packed: each read at its own length, ceil(len / 32) words
+            PG_CUDA(cudaStreamSynchronize(st_));
+            check_format(h_cnt_);
+            std::vector<u64> ofs(n);
+            n_words = 0;
+            for (u64 r = 0; r < n; r++) { ofs[r] = n_words; n_words += ((*lens)[l0 + r] + 31) / 32; }
+            pack_ofs_.ensure(n * sizeof(u64));
+            pack_words_.ensure(n_words * sizeof(u64) + 8);
+            PG_CUDA(cudaMemcpyAsync(pack_ofs_.p, ofs.data(), n * sizeof(u64), cudaMemcpyHostToDevice, st_));
+            k_pack_reads<<<(unsigned)std::min<u64>((n + 7) / 8, (u64)n_sm_ * 16), 256, 0, st_>>>(src, S, read_lens_.as<u32>(), pack_ofs_.as<u64>(), n,
+                                                                                                 pack_words_.as<u64>());
+            PG_CUDA(cudaGetLastError());
+            PG_CUDA(cudaEventRecord(ev_[1], st_));
+            src = pack_words_.as<u64>();
+        }
+        words->resize(w0 + n_words);
+        PG_CUDA(cudaMemcpyAsync(words->data() + w0, src, n_words * sizeof(u64), cudaMemcpyDeviceToHost, st_));
         PG_CUDA(cudaStreamSynchronize(st_));
         check_format(h_cnt_);
         float ms;
@@ -278,17 +385,53 @@ public:
         PG_CUDA(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
         ms_scan_ += ms;
     }
-    void times(double* ms_hash, double* ms_decode, double* ms_scan) const override { *ms_hash = ms_hash_; *ms_decode = ms_decode_; *ms_scan = ms_scan_; }
+
+    void map_long_batch(const u64* words, u64 n_words, const u64* wofs, const u32* lens, u64 n, int alignlen, MapHit* out) override {
+        PG_CUDA(cudaSetDevice(device_));
+        std::vector<u64> kofs(n + 1);
+        u64 k = 0;
+        for (u64 r = 0; r < n; r++) { kofs[r] = k; if ((int)lens[r] >= K_ + 1) k += lens[r] - K_ + 1; }
+        kofs[n] = k;
+        batch_words_.ensure(n_words * sizeof(u64) + 8);
+        batch_wofs_.ensure(n * sizeof(u64) + 8);
+        batch_lens_.ensure(n * sizeof(u32) + 4);
+        batch_kofs_.ensure((n + 1) * sizeof(u64));
+        hits_.ensure(k * sizeof(u64) + 8);
+        out_.ensure(n * sizeof(MapHit) + 16);
+        PG_CUDA(cudaMemcpyAsync(batch_words_.p, words, n_words * sizeof(u64), cudaMemcpyHostToDevice, st_));
+        PG_CUDA(cudaMemcpyAsync(batch_wofs_.p, wofs, n * sizeof(u64), cudaMemcpyHostToDevice, st_));
+        PG_CUDA(cudaMemcpyAsync(batch_lens_.p, lens, n * sizeof(u32), cudaMemcpyHostToDevice, st_));
+        PG_CUDA(cudaMemcpyAsync(batch_kofs_.p, kofs.data(), (n + 1) * sizeof(u64), cudaMemcpyHostToDevice, st_));
+        PG_CUDA(cudaEventRecord(ev_[0], st_));
+        if (n) {
+            k_map_long<NW><<<(unsigned)std::min<u64>(n, (u64)n_sm_ * 16), MAP_LONG_THREADS, 0, st_>>>(tab_, kp_, batch_words_.as<u64>(), batch_wofs_.as<u64>(),
+                                                                                                       batch_lens_.as<u32>(), batch_kofs_.as<u64>(), n, alignlen,
+                                                                                                       n_groups_, hits_.as<u64>(), out_.as<MapHit>());
+            PG_CUDA(cudaGetLastError());
+        }
+        PG_CUDA(cudaEventRecord(ev_[1], st_));
+        PG_CUDA(cudaMemcpyAsync(out, out_.p, n * sizeof(MapHit), cudaMemcpyDeviceToHost, st_));
+        PG_CUDA(cudaStreamSynchronize(st_));
+        float ms;
+        PG_CUDA(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
+        ms_long_ += ms;
+        lookups_long_ += k;
+    }
+    void times(MapTimes* t) const override { *t = MapTimes{ms_hash_, ms_decode_, ms_scan_, ms_long_, lookups_long_}; }
 
 private:
     int K_, device_, W64_ = 1, n_sm_ = 0;
+    // group slots of k_map_long; PGB200_MAP_GROUPS lowers it (1..MAP_GROUPS) so that a test can force the overflow rounds
+    u32 n_groups_ = getenv("PGB200_MAP_GROUPS") ? (u32)std::min<long>(std::max<long>(1, atol(getenv("PGB200_MAP_GROUPS"))), (long)MAP_GROUPS) : MAP_GROUPS;
     KParams<NW> kp_;
     Stream st_;
     Event ev_[2];
     Pinned<u64> h_cnt_;
-    DevBuf cnt_, tab_buf_, text_buf_, scan_buf_, line_buf_, read_words_, read_lens_, batch_words_, batch_lens_, batch_kofs_, hits_, out_;
+    DevBuf cnt_, tab_buf_, text_buf_, scan_buf_, line_buf_, read_words_, read_lens_, pack_ofs_, pack_words_, batch_words_, batch_wofs_, batch_lens_,
+        batch_kofs_, hits_, out_;
     Table<NW> tab_{nullptr, 0};
-    double ms_hash_ = 0, ms_decode_ = 0, ms_scan_ = 0;
+    double ms_hash_ = 0, ms_decode_ = 0, ms_scan_ = 0, ms_long_ = 0;
+    u64 lookups_long_ = 0;
 };
 
 IMapEngine* make_map_engine(int K, int device, int max_rd_len) {

@@ -4,10 +4,14 @@
 //   prlContig2nodes (host part)            prlHashCtg.c:325-467   (.contig parsing, which contigs are kept, their ids)
 //   basicContigInfo                        prlRead2Ctg.c:727-763  (.ContigIndex -> lengths, bal_edge)
 //   prlRead2Ctg / recordAlldgn / getReadIngap / output1read_gz / getPEreadOnContig   prlRead2Ctg.c:427-712, 779-1053
+//   prlLongRead2Ctg / recordLongRead / output1read         prlRead2Ctg.c:456-492, 612-625, 1080-1298
 // The k-mer work (contig table, read scan, parse1read) runs on the GPU (map.cu); the .contig text is parsed here, on the host: it is a
 // few hundred MB at most, multi-line, and is read once.
 //
-// Long-read libraries (asm_flags=4, prlLongRead2Ctg) and BAM are refused before any output is written.  locate1read
+// Long-read libraries (asm_flags=4) are mapped first, when getMaxLongReadLen >= 1, and write .longReadInGap (.RlongReadInGap with
+// -f); configs without them give the same output and stderr as a stage without the long pass.  Both passes' reads are decoded
+// before any output file is opened, so every refusal -- BAM, two-file pairs in a long library, a read that would overflow the
+// reference's read buffers -- comes before the first output.  locate1read
 // (prlRead2Ctg.c:389-425) is not restated: recordAlldgn calls it only for a read with footprint set whose contig id is < 1, but
 // parse1read sets footprint only after it chose a contig, and a chosen contig id is either atoi(name) > 0, an ordinal >= 1, or its
 // twin id, which is >= 1 as well.
@@ -146,7 +150,6 @@ ContigInfo contig_info(const std::string& prefix) {
     ContigInfo ci;
     int num_long = 0, index, length, bal;
     if (fgets(line, sizeof line, fp) && strlen(line) > 8) sscanf(line + 8, "%d %d", &ci.num_all, &num_long);
-    fprintf(stderr, "%d edge(s) in the graph.\n", ci.num_all);
     ci.length.assign((size_t)std::max(ci.num_all, 0) + 1, 0);
     ci.bal_edge.assign(ci.length.size(), 0);
     if (!fgets(line, sizeof line, fp)) line[0] = 0;
@@ -165,13 +168,14 @@ ContigInfo contig_info(const std::string& prefix) {
     return ci;
 }
 
-// All map reads, in the order read1seqInLib returns them (mates interleaved), packed W64 words per read
+// The reads of one pass, in the order read1seqInLib returns them (short pass: mates interleaved, W64 words per read; long pass: each
+// read packed at its own length, at wofs[r])
 struct Reads {
-    std::vector<u64> words;
+    std::vector<u64> words, wofs;
     std::vector<u32> lens;
-    std::vector<int> lib;   // index into MapPlan::libs
+    std::vector<int> lib;   // index into MapPlan::libs / long_libs
 };
-void decode_file(IMapEngine& eng, const PlanEntry& f, std::vector<u64>* words, std::vector<u32>* lens) {
+void decode_file(IMapEngine& eng, const PlanEntry& f, int maxlen, int stride, std::vector<u64>* words, std::vector<u32>* lens) {
     std::unique_ptr<FILE, int (*)(FILE*)> file(fopen(f.path.c_str(), "rb"), fclose);
     if (!file) fail("Cannot open %s. Now exit to system...", f.path.c_str());
     const size_t cap = (size_t)(getenv("PGB200_CHUNK_MB") ? atoi(getenv("PGB200_CHUNK_MB")) : 256) << 20;
@@ -194,12 +198,75 @@ void decode_file(IMapEngine& eng, const PlanEntry& f, std::vector<u64>* words, s
             if (cut == 0 && have == cap) fail("pgb200: a single record exceeds the %zu MB chunk", cap >> 20);
             if (cut == 0) continue;
         }
-        try { eng.decode_text(buf.data(), cut, f.fastq, f.reverse, f.cut, words, lens); }
+        try { eng.decode_text(buf.data(), cut, f.fastq, f.reverse, maxlen, stride, words, lens); }
         catch (const std::exception& ex) { fail("readseqInLib return error! please make sure input file is correct fastq/fasta file \n(%s)", ex.what()); }
         memmove(buf.data(), buf.data() + cut, have - cut);
         have -= cut;
     }
 }
+
+// One pass's reads, decoded before anything is written: every refusal comes before the first output file.  The stderr lines the
+// reference prints while it reads go to *log, to be printed where the pass prints them.  A read longer than `room` would run past
+// the reference's seqBuffer (allocated for `room` bases): no output is defined for it, so it is refused.  Each file is decoded
+// with one base of slack past `room` so that such a read shows.
+Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pass, int room, int stride, std::string* log) {
+    Reads rd;
+    char line[256];
+    auto say = [&](const char* fmt, auto... a) { snprintf(line, sizeof line, fmt, a...); *log += line; };
+    for (size_t li = 0; li < libs.size(); li++) {
+        const MapLib& L = libs[li];
+        const size_t lib_begin = rd.lens.size();
+        for (size_t fi = 0; fi < L.files.size(); fi++) {
+            const PlanEntry& e = L.files[fi];
+            const int maxlen = std::min(e.cut, room + 1);
+            const size_t before = rd.lens.size();
+            if (e.mate == 0) {
+                // openFileInLib names both mates before the first read; mates then alternate r1, r2, r1, r2
+                const PlanEntry& m = L.files[++fi];
+                say("Import reads from file:\n %s\n", e.path.c_str());
+                say("Import reads from file:\n %s\n", m.path.c_str());
+                std::vector<u64> w1, w2;
+                std::vector<u32> l1, l2;
+                decode_file(eng, e, maxlen, stride, &w1, &l1);
+                decode_file(eng, m, maxlen, stride, &w2, &l2);
+                if (l1.size() != l2.size())
+                    fail("pgb200: mate files hold different numbers of reads (%zu vs %zu): unsupported", l1.size(), l2.size());
+                rd.words.resize(rd.words.size() + 2 * w1.size());
+                u64* dst = rd.words.data() + before * stride;
+                for (size_t r = 0; r < l1.size(); r++) {
+                    memcpy(dst + (2 * r) * stride, w1.data() + r * stride, stride * sizeof(u64));
+                    memcpy(dst + (2 * r + 1) * stride, w2.data() + r * stride, stride * sizeof(u64));
+                    rd.lens.push_back(l1[r]);
+                    rd.lens.push_back(l2[r]);
+                }
+            } else {
+                say("Import reads from file:\n %s\n", e.path.c_str());
+                decode_file(eng, e, maxlen, stride, &rd.words, &rd.lens);
+            }
+            for (size_t r = before; r < rd.lens.size(); r++)
+                if ((int)rd.lens[r] > room)
+                    fail("pgb200: %s holds a read longer than %d bases (%s); the reference would write past its read buffer", e.path.c_str(), room,
+                         long_pass ? "the long-read length, getMaxLongReadLen"
+                                   : "max_rd_len: the long-read libraries raise the short reads' length cutoff to maxReadLen4all");
+            rd.lib.resize(rd.lens.size(), (int)li);
+            if (rd.lens.size() > before && lib_begin == before) {
+                if (long_pass) say("Map_len %d.\n", std::max(L.map_len, 35));   // prlRead2Ctg.c:1198-1204
+                else say("Current insert size is %d, map_len is %d.\n", L.avg_ins, L.avg_ins > 1000 ? std::max(L.map_len, 35) : std::max(L.map_len, 32));   // :903-919
+            }
+            for (size_t r = before; r < rd.lens.size(); r++)
+                if ((r + 1) % 100000000 == 0) say("--- %lldth reads.\n", (long long)(r + 1));
+        }
+    }
+    if (stride == 0) {   // packed reads: word offsets from the lengths
+        rd.wofs.resize(rd.lens.size() + 1);
+        u64 o = 0;
+        for (size_t r = 0; r < rd.lens.size(); r++) { rd.wofs[r] = o; o += (rd.lens[r] + 31) / 32; }
+        rd.wofs.back() = o;
+    }
+    return rd;
+}
+
+template <class T> void put(std::string& s, const T& v) { s.append(reinterpret_cast<const char*>(&v), sizeof v); }
 
 struct RcSeqModel {
     std::vector<unsigned char> b;
@@ -211,7 +278,117 @@ struct RcSeqModel {
             x = (unsigned char)((x & ~(3u << sh)) | (c << sh));
         }
     }
+    // thread 0's chops of a batch of n reads leave their reverse complements here (chopKmer4read, prlRead2Ctg.c:153-187): reads
+    // t = 0 (mod P) with len >= K+1, the later ones over the earlier ones
+    template <class WordsOf>
+    void chops(u64 n, int P, int K, const u32* lens, WordsOf words_of) {
+        size_t covered = 0;
+        for (long long t = ((long long)n - 1) / P * P; t >= 0 && covered < b.size(); t -= P) {
+            const int len = (int)lens[t];
+            if (len < K + 1 || (size_t)len <= covered) continue;
+            const u64* w = words_of((u64)t);
+            for (size_t i = covered; i < (size_t)len; i++) {
+                const int src = len - 1 - (int)i;
+                b[i] = (unsigned char)((((w[src >> 5] >> (2 * (src & 31))) & 3u)) ^ 2u);
+            }
+            covered = (size_t)len;
+        }
+    }
 };
+
+// parse1read's output arrays for one batch: the contig lengths and twins applied to the GPU's placements
+struct Placement {
+    std::vector<u32> ctg;
+    std::vector<int> pos;
+    std::vector<char> orien, footprint;
+    explicit Placement(size_t n) : ctg(n), pos(n), orien(n, 0), footprint(n) {}
+    void set(const MapHit* hit, u64 n, const ContigInfo& ci, int K, const std::string& prefix) {
+        for (u64 t = 0; t < n; t++) {
+            const MapHit& h = hit[t];
+            footprint[t] = (h.flags & MAP_FOOTPRINT) ? 1 : 0;
+            if (!(h.flags & MAP_PLACED)) { ctg[t] = 0; continue; }
+            if (h.ctg >= ci.length.size()) fail("pgb200: contig %u is not in %s.ContigIndex", h.ctg, prefix.c_str());
+            const u32 len = ci.length[h.ctg];
+            if (h.flags & MAP_MINUS) {
+                orien[t] = '-';
+                ctg[t] = h.ctg + (u32)ci.bal_edge[h.ctg] - 1u;   // getTwinCtg, attachPEinfo.c:666-669
+                pos[t] = (int)(len - (u32)h.node_pos - (u32)K - (u32)h.i + 1u);
+            } else {
+                orien[t] = '+';
+                ctg[t] = h.ctg;
+                pos[t] = (int)((u32)h.node_pos - (u32)h.i + 1u);
+            }
+        }
+    }
+};
+
+long long batch_reads(const char* what, int read_len, int K) {   // maxReadNum, prlRead2Ctg.c:814-815 and 1115-1116
+    if (read_len - K + 1 <= 0) fail("pgb200: %s %d is shorter than K %d", what, read_len, K);
+    long long m = 100000000 / (read_len - K + 1);
+    if (m % 2) m--;
+    if (m < 2) fail("pgb200: %s %d leaves no room for a read pair in a batch", what, read_len);
+    return m;
+}
+
+void print_libs(const MapPlan& plan) {   // free_libs, lib.c:516-520
+    fprintf(stderr, "LIB(s) information:\n");
+    for (size_t i = 0; i < plan.libs.size(); i++) fprintf(stderr, " [LIB] %zu, avg_ins %d, reverse %d.\n", i, plan.libs[i].avg_ins, plan.libs[i].reverse);
+}
+
+// prlLongRead2Ctg once its reads are in: batches of maxReadNum reads (from longReadLen), parse1read on the GPU (k_map_long), and
+// recordLongRead / output1read here.  Every long read has insert size 18; a read whose footprint is set goes to .longReadInGap (len,
+// contig, pos and its bases packed from this pass's own rcSeq[1], a zeroed buffer of longReadLen bytes) and, with -f, as text to
+// .RlongReadInGap.  Both are plain files.
+void map_long_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, long long max_read_num, const ContigInfo& ci, int K, int P, int fill,
+                    const std::string& prefix) {
+    const u64 n_reads = rd.lens.size();
+    std::vector<MapHit> hit((size_t)std::min<long long>(max_read_num, (long long)std::max<u64>(n_reads, 1)));
+    Placement pl(hit.size());
+    RcSeqModel rc{std::vector<unsigned char>((size_t)plan.long_len, 0)};
+    std::unique_ptr<FILE, int (*)(FILE*)> f_gap(ckopen(prefix + ".longReadInGap", "wb"), fclose);
+    std::unique_ptr<FILE, int (*)(FILE*)> f_txt(fill ? ckopen(prefix + ".RlongReadInGap", "w") : nullptr, fclose);
+    auto put_file = [&](FILE* f, const std::string& s, const char* suffix) {
+        if (!s.empty() && fwrite(s.data(), 1, s.size(), f) != s.size()) fail("short write on %s%s", prefix.c_str(), suffix);
+    };
+    long long read_counter = 0, in_gap = 0, last_batch = 0;
+    std::vector<u64> wofs;
+    std::string s_gap, s_txt;
+    char line[128];
+    for (u64 b0 = 0; b0 < n_reads; b0 += (u64)max_read_num) {
+        const u64 n = std::min<u64>((u64)max_read_num, n_reads - b0);
+        last_batch = (long long)n;
+        const int alignlen = std::max(plan.long_libs[rd.lib[b0 + n - 1]].map_len, 35);   // ALIGNLEN after the batch's last read (:1198-1204)
+        const u64 w0 = rd.wofs[b0];
+        wofs.resize(n);
+        for (u64 t = 0; t < n; t++) wofs[t] = rd.wofs[b0 + t] - w0;
+        const u64* W = rd.words.data() + w0;
+        const u32* Ln = rd.lens.data() + b0;
+        try { eng.map_long_batch(W, rd.wofs[b0 + n] - w0, wofs.data(), Ln, n, alignlen, hit.data()); }
+        catch (const std::exception& ex) { fail("pgb200: long-read scan failed: %s", ex.what()); }
+        rc.chops(n, P, K, Ln, [&](u64 t) { return W + wofs[t]; });
+        pl.set(hit.data(), n, ci, K, prefix);
+        s_gap.clear(); s_txt.clear();
+        for (u64 t = 0; t < n; t++) {   // recordLongRead, output1read (prlRead2Ctg.c:456-492, 612-625)
+            read_counter++;
+            if (!pl.footprint[t]) continue;
+            const int len = (int)Ln[t];
+            const u64* w = W + wofs[t];
+            in_gap++;
+            rc.tight(w, len);
+            put(s_gap, len); put(s_gap, (int)pl.ctg[t]); put(s_gap, pl.pos[t]);
+            s_gap.append(reinterpret_cast<const char*>(rc.b.data()), (size_t)(len / 4 + 1));
+            if (fill && len > 0) {
+                s_txt.append(line, (size_t)snprintf(line, sizeof line, ">%d\t%d\t%d\t%c\t%d\t%d\n", len, (int)pl.ctg[t], pl.pos[t], pl.orien[t], 18, 0));
+                for (int i = 0; i < len; i++) s_txt.push_back("ACTG"[(w[i >> 5] >> (2 * (i & 31))) & 3]);
+                s_txt.push_back('\n');
+            }
+        }
+        put_file(f_gap.get(), s_gap, ".longReadInGap");
+        if (fill) put_file(f_txt.get(), s_txt, ".RlongReadInGap");
+    }
+    if (n_reads && last_batch != max_read_num)   // a batch that ends exactly at the last read is recorded inside the reference's loop
+        fprintf(stderr, "Output %lld out of %lld (%.1f)%% reads in gaps.\n", in_gap, read_counter, (float)in_gap / read_counter * 100);
+}
 
 struct GzOut {
     gzFile f = nullptr;
@@ -228,7 +405,6 @@ struct GzOut {
     void close() { if (f) gzclose(f); f = nullptr; }
     ~GzOut() { close(); }
 };
-template <class T> void put(std::string& s, const T& v) { s.append(reinterpret_cast<const char*>(&v), sizeof v); }
 
 int map_stage(int argc, char** argv, int flavour127) {
     const double t_all = host_now();
@@ -272,8 +448,13 @@ int map_stage(int argc, char** argv, int flavour127) {
     // the plan is read before the engine so that a refused library stops the stage before any output
     const MapPlan plan = map_plan(cfg.c_str());
     if (plan.max_rd_len - K + 1 <= 0) fail("pgb200: max_rd_len %d is shorter than K %d", plan.max_rd_len, K);
+    const bool long_pass = plan.long_len >= 1;   // prlRead2Ctg.c:1099-1104
+    // the short reads' stride holds max_rd_len bases, and one more where the long pass raises a cutoff past max_rd_len (load_reads)
+    int short_len = plan.max_rd_len;
+    for (const MapLib& L : plan.libs)
+        for (const PlanEntry& e : L.files) short_len = std::max(short_len, std::min(e.cut, plan.max_rd_len + 1));
     std::unique_ptr<IMapEngine> eng;
-    try { eng.reset(make_map_engine(K, device, plan.max_rd_len)); } catch (const std::exception& ex) { fail("pgb200: %s", ex.what()); }
+    try { eng.reset(make_map_engine(K, device, short_len)); } catch (const std::exception& ex) { fail("pgb200: %s", ex.what()); }
     const double t_hash = host_now();
     u64 distinct = 0;
     try { eng->hash_contigs(ctg.packed.data(), ctg.off.back(), ctg.off.data(), ctg.id.data(), ctg.id.size(), &distinct); }
@@ -281,75 +462,71 @@ int map_stage(int argc, char** argv, int flavour127) {
     fprintf(stderr, "Time spent on hashing contigs: %ds.\n", (int)((host_now() - t_hash) * 1e-3));
     fprintf(stderr, "%lli node(s) allocated, %lli kmer(s) in contigs, %lli kmer(s) processed.\n", (long long)distinct, (long long)ctg.n_kmers, (long long)ctg.n_kmers);
     fprintf(stderr, "Time spent on graph construction: %ds.\n\n", (int)((host_now() - t0) * 1e-3));
-    fprintf(stderr, "Time spent on aligning long reads: %ds.\n\n", 0);
+
+    // ---- the reads of both passes, before any output file
+    t0 = host_now();
+    const int W64 = eng->words_per_read();
+    std::string long_log, short_log;
+    const Reads lrd = long_pass ? load_reads(*eng, plan.long_libs, true, plan.long_len, 0, &long_log) : Reads{};
+    const Reads rd = load_reads(*eng, plan.libs, false, plan.max_rd_len, W64, &short_log);
+    const double ms_read = host_now() - t0;
+    const long long max_read_num = batch_reads("max_rd_len", plan.max_rd_len, K);
+    const long long max_long_num = long_pass ? batch_reads("long read length", plan.long_len, K) : 0;
+    const char* long_env = getenv("PGB200_MAP_LONG");
+    const bool long_all = long_env && !strcmp(long_env, "all");   // the short pass through k_map_long too: a second exact implementation
+
+    // ---- prlLongRead2Ctg
+    ContigInfo ci;
+    t0 = host_now();
+    if (long_pass) {
+        fprintf(stderr, "In file: %s, long read len %d, max name len %d.\n", cfg.c_str(), plan.long_len, 256);
+        fprintf(stderr, "%d thread(s) initialized.\n", P);
+        ci = contig_info(prefix);   // basicContigInfo runs once: here, not in the short pass
+        fprintf(stderr, "%d edge(s) in the graph.\n", ci.num_all);
+        fputs(long_log.c_str(), stderr);
+        map_long_reads(*eng, plan, lrd, max_long_num, ci, K, P, fill, prefix);
+        print_libs(plan);
+        fprintf(stderr, "0 reads deleted.\n");
+        if (verbose) {
+            MapTimes tm;
+            eng->times(&tm);
+            fprintf(stderr, "[pgb200] map long pass: %zu reads, %.0f ms (host), long-read scan %.1f ms (GPU events), %llu lookups\n", lrd.lens.size(),
+                    host_now() - t0, tm.ms_long, (unsigned long long)tm.lookups_long);
+        }
+    }
+    fprintf(stderr, "Time spent on aligning long reads: %ds.\n\n", (int)((host_now() - t0) * 1e-3));
 
     // ---- prlRead2Ctg
     t0 = host_now();
     fprintf(stderr, "In file: %s, max seq len %d, max name len %d\n", cfg.c_str(), plan.max_rd_len, 256);
     fprintf(stderr, "%d thread(s) initialized.\n", P);
-    const ContigInfo ci = contig_info(prefix);
+    if (!long_pass) {
+        ci = contig_info(prefix);
+        fprintf(stderr, "%d edge(s) in the graph.\n", ci.num_all);
+    }
     GzOut f_gap, f_short, f_on, f_pe;
     f_gap.open(prefix + ".readInGap.gz", "wb");
     if (fill) f_short.open(prefix + ".shortreadInGap.gz", "w");
     f_on.open(prefix + ".readOnContig.gz", "w");
     if (fill) f_pe.open(prefix + ".PEreadOnContig.gz", "wb");
     f_on.write("read\tcontig\tpos\n");
-
-    const int W64 = eng->words_per_read();
-    Reads rd;
+    fputs(short_log.c_str(), stderr);
     struct Grad { int ins; long long bound; int rank, cut; };
-    std::vector<Grad> grads;
-    for (size_t li = 0; li < plan.libs.size(); li++) {
-        const MapLib& L = plan.libs[li];
-        const size_t lib_begin = rd.lens.size();
-        for (size_t fi = 0; fi < L.files.size(); fi++) {
-            const PlanEntry& e = L.files[fi];
-            const size_t before = rd.lens.size();
-            if (e.mate == 0) {
-                // openFileInLib names both mates before the first read; mates then alternate r1, r2, r1, r2
-                const PlanEntry& m = L.files[++fi];
-                fprintf(stderr, "Import reads from file:\n %s\n", e.path.c_str());
-                fprintf(stderr, "Import reads from file:\n %s\n", m.path.c_str());
-                std::vector<u64> w1, w2;
-                std::vector<u32> l1, l2;
-                decode_file(*eng, e, &w1, &l1);
-                decode_file(*eng, m, &w2, &l2);
-                if (l1.size() != l2.size())
-                    fail("pgb200: mate files hold different numbers of reads (%zu vs %zu): unsupported", l1.size(), l2.size());
-                rd.words.resize(rd.words.size() + 2 * w1.size());
-                u64* dst = rd.words.data() + before * W64;
-                for (size_t r = 0; r < l1.size(); r++) {
-                    memcpy(dst + (2 * r) * W64, w1.data() + r * W64, W64 * sizeof(u64));
-                    memcpy(dst + (2 * r + 1) * W64, w2.data() + r * W64, W64 * sizeof(u64));
-                    rd.lens.push_back(l1[r]);
-                    rd.lens.push_back(l2[r]);
-                }
-            } else {
-                fprintf(stderr, "Import reads from file:\n %s\n", e.path.c_str());
-                decode_file(*eng, e, &rd.words, &rd.lens);
-            }
-            rd.lib.resize(rd.lens.size(), (int)li);
-            if (rd.lens.size() > before && lib_begin == before) {
-                int al = L.map_len;   // prlRead2Ctg.c:903-919
-                al = L.avg_ins > 1000 ? std::max(al, 35) : std::max(al, 32);
-                fprintf(stderr, "Current insert size is %d, map_len is %d.\n", L.avg_ins, al);
-            }
-            for (size_t r = before; r < rd.lens.size(); r++)
-                if ((r + 1) % 100000000 == 0) fprintf(stderr, "--- %lldth reads.\n", (long long)(r + 1));
+    std::vector<Grad> grads;   // a library's boundary is the count of reads up to its last one (readseq1by1.c:1092-1102)
+    for (size_t r = 0; r < rd.lens.size(); r++)
+        if (r + 1 == rd.lens.size() || rd.lib[r + 1] != rd.lib[r]) {
+            const MapLib& L = plan.libs[rd.lib[r]];
+            grads.push_back({L.avg_ins, (long long)r + 1, L.rank, L.pair_num_cut});
         }
-        if (rd.lens.size() > lib_begin) grads.push_back({L.avg_ins, (long long)rd.lens.size(), L.rank, L.pair_num_cut});   // readseq1by1.c:1092-1102
-    }
     const u64 n_reads = rd.lens.size();
-    const double ms_read = host_now() - t0;
 
-    // ---- batches of maxReadNum reads (prlRead2Ctg.c:814-815), parse1read on the GPU, recordAlldgn here
-    long long max_read_num = 100000000 / (plan.max_rd_len - K + 1);
-    if (max_read_num % 2) max_read_num--;
-    if (max_read_num < 2) fail("pgb200: max_rd_len %d leaves no room for a read pair in a batch", plan.max_rd_len);
+    // ---- batches of maxReadNum reads, parse1read on the GPU, recordAlldgn here
     std::vector<MapHit> hit((size_t)std::min<long long>(max_read_num, (long long)std::max<u64>(n_reads, 1)));
-    std::vector<u32> ctg_arr(hit.size());
-    std::vector<int> pos_arr(hit.size());
-    std::vector<char> orien(hit.size(), 0), footprint(hit.size());
+    Placement pl(hit.size());
+    std::vector<u32>& ctg_arr = pl.ctg;
+    std::vector<int>& pos_arr = pl.pos;
+    std::vector<char>&orien = pl.orien, &footprint = pl.footprint;
+    std::vector<u64> wofs;
     RcSeqModel rc{std::vector<unsigned char>((size_t)plan.max_rd_len, 0)};
     long long read_counter = 0, map_counter = 0, in_gap = 0;
     int alignlen = 0, prev_lib = -1;
@@ -370,38 +547,16 @@ int map_stage(int argc, char** argv, int flavour127) {
         }
         const u64* W = rd.words.data() + b0 * W64;
         const u32* Ln = rd.lens.data() + b0;
-        try { eng->map_batch(W, Ln, n, alignlen, hit.data()); } catch (const std::exception& ex) { fail("pgb200: read scan failed: %s", ex.what()); }
+        try {
+            if (long_all) {   // PGB200_MAP_LONG=all: the same batch through k_map_long
+                wofs.resize(n);
+                for (u64 t = 0; t < n; t++) wofs[t] = t * W64;
+                eng->map_long_batch(W, n * W64, wofs.data(), Ln, n, alignlen, hit.data());
+            } else eng->map_batch(W, Ln, n, alignlen, hit.data());
+        } catch (const std::exception& ex) { fail("pgb200: read scan failed: %s", ex.what()); }
         const double t_rec = host_now();
-        // thread 0's chops of this batch leave their reverse complements in rcSeq[1] (chopKmer4read, prlRead2Ctg.c:153-187)
-        {
-            size_t covered = 0;
-            for (long long t = ((long long)n - 1) / P * P; t >= 0 && covered < rc.b.size(); t -= P) {
-                const int len = (int)Ln[t];
-                if (len < K + 1 || (size_t)len <= covered) continue;
-                const u64* w = W + (u64)t * W64;
-                for (size_t i = covered; i < (size_t)len; i++) {
-                    const int src = len - 1 - (int)i;
-                    rc.b[i] = (unsigned char)((((w[src >> 5] >> (2 * (src & 31))) & 3u)) ^ 2u);
-                }
-                covered = (size_t)len;
-            }
-        }
-        for (u64 t = 0; t < n; t++) {   // the reads' placements: parse1read's output arrays
-            const MapHit& h = hit[t];
-            footprint[t] = (h.flags & MAP_FOOTPRINT) ? 1 : 0;
-            if (!(h.flags & MAP_PLACED)) { ctg_arr[t] = 0; continue; }
-            if (h.ctg >= ci.length.size()) fail("pgb200: contig %u is not in %s.ContigIndex", h.ctg, prefix.c_str());
-            const u32 len = ci.length[h.ctg];
-            if (h.flags & MAP_MINUS) {
-                orien[t] = '-';
-                ctg_arr[t] = h.ctg + (u32)ci.bal_edge[h.ctg] - 1u;   // getTwinCtg, attachPEinfo.c:666-669
-                pos_arr[t] = (int)(len - (u32)h.node_pos - (u32)K - (u32)h.i + 1u);
-            } else {
-                orien[t] = '+';
-                ctg_arr[t] = h.ctg;
-                pos_arr[t] = (int)((u32)h.node_pos - (u32)h.i + 1u);
-            }
-        }
+        rc.chops(n, P, K, Ln, [&](u64 t) { return W + t * W64; });
+        pl.set(hit.data(), n, ci, K, prefix);
         // recordAlldgn (prlRead2Ctg.c:627-712) into this batch's byte strings
         const double t_join = host_now();
         if (writer.joinable()) writer.join();
@@ -481,22 +636,21 @@ int map_stage(int argc, char** argv, int flavour127) {
     f_on.close();
     {
         FILE* fo = ckopen(prefix + ".peGrads", "w");
-        fprintf(fo, "grads&num: %d\t%lld\t%d\n", (int)grads.size(), (long long)n_reads, plan.max_rd_len);
+        fprintf(fo, "grads&num: %d\t%lld\t%d\n", (int)grads.size(), (long long)n_reads, plan.max_len4all);
         if (!grads.empty()) fprintf(stderr, "%d pe insert size, the largest boundary is %lld.\n\n", (int)grads.size(), grads.back().bound);
         else fprintf(stderr, "No paired reads found.\n");
         for (const Grad& g : grads) fprintf(fo, "%d\t%lld\t%d\t%d\n", g.ins, g.bound, g.rank, g.cut);
         fclose(fo);
     }
     f_gap.close(); f_short.close(); f_pe.close();
-    fprintf(stderr, "LIB(s) information:\n");
-    for (size_t i = 0; i < plan.libs.size(); i++) fprintf(stderr, " [LIB] %zu, avg_ins %d, reverse %d.\n", i, plan.libs[i].avg_ins, plan.libs[i].reverse);
+    print_libs(plan);
     fprintf(stderr, "Time spent on aligning reads: %ds.\n\n", (int)((host_now() - t0) * 1e-3));
     if (verbose) {
-        double ms_hash, ms_decode, ms_scan;
-        eng->times(&ms_hash, &ms_decode, &ms_scan);
+        MapTimes tm;
+        eng->times(&tm);
         fprintf(stderr, "[pgb200] map: parse .contig %.0f ms (host), contig hash %.1f ms, read decode %.1f ms, read scan %.1f ms (GPU events); reading %.0f ms, "
                         "record pass %.0f ms, waiting for the deflate %.0f ms (host)\n",
-                ms_parse, ms_hash, ms_decode, ms_scan, ms_read, ms_record, ms_deflate);
+                ms_parse, tm.ms_hash, tm.ms_decode, long_all ? tm.ms_long : tm.ms_scan, ms_read, ms_record, ms_deflate);
     }
     eng.reset();
     fprintf(stderr, "Overall time spent on alignment: %dm.\n\n", (int)((host_now() - t_all) * 1e-3) / 60);

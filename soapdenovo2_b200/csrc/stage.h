@@ -23,9 +23,12 @@ struct PlanEntry { std::string path; bool fastq; int mate, reverse, cut; };
 struct ReadPlan { int n_libs, max_rd_len; std::vector<PlanEntry> files; };
 ReadPlan read_plan(const char* cfg);
 // The map stage's plan: every library in config order after the sort by avg_ins, with the files map reads (paired ones, asm_flags 2|3)
+// MapPlan::long_libs: the asm_flags=4 libraries (prlLongRead2Ctg), their p, f, q files in that order, each read cut to `cut` bases.
+// long_len is getMaxLongReadLen (0: no long pass); the libraries' `cut` and the short pass's use max_len4all = max(max_rd_len,
+// long_len).
 struct MapLib { int avg_ins, reverse, map_len, rank, pair_num_cut; std::vector<PlanEntry> files; };
-struct MapPlan { int max_rd_len; std::vector<MapLib> libs; };
-MapPlan map_plan(const char* cfg);   // refuses asm_flags=4 and b= libraries
+struct MapPlan { int max_rd_len, long_len = 0, max_len4all = 0; std::vector<MapLib> libs, long_libs; };
+MapPlan map_plan(const char* cfg);   // refuses b= libraries and two-file pairs in asm_flags=4 libraries
 size_t last_record_start(const char* buf, size_t n, bool fastq);   // the chunk cutter
 void write_file(const std::string& name, const void* data, size_t n);
 void write_kmer_freq(const std::string& prefix, const long long hist[256]);

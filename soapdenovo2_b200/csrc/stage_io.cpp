@@ -99,15 +99,34 @@ ReadPlan read_plan(const char* cfg) {
     return plan;
 }
 
-// The map stage reads with pair = 1 and asm_ctg = 0 (prlRead2Ctg.c:887, readseq1by1.c:595-674): libraries with asm_flags 2|3, and
-// inside each only the f1/f2 pairs, q1/q2 pairs and p files.  Every library is kept for the "LIB(s) information" lines.
+// The map stage reads twice.  The long pass (prlLongRead2Ctg) reads with pair = 0 and asm_ctg = 4: the asm_flags=4 libraries, and
+// inside each the p, f and q files (two-file pairs are refused: read unpaired they would be mates taken as single reads).  The short
+// pass reads with pair = 1 and asm_ctg = 0 (prlRead2Ctg.c:887, readseq1by1.c:595-674): libraries with asm_flags 2|3, and inside each
+// only the f1/f2 pairs, q1/q2 pairs and p files.  Every library is kept for the "LIB(s) information" lines.  Each read is cut to
+// min(rd_len_cutoff, maxReadLen4all), or maxReadLen4all without a cutoff (readseq1by1.c:1083-1090); maxReadLen4all is max_rd_len
+// raised to longReadLen by the long pass (prlRead2Ctg.c:1106).
 MapPlan map_plan(const char* cfg) {
     MapPlan plan;
     const std::vector<Lib> libs = scan_lib(cfg, &plan.max_rd_len);
+    bool has_long = false;
+    for (const Lib& L : libs) {   // getMaxLongReadLen, lib.c:43-68
+        if (L.asm_flag != 4) continue;
+        has_long = true;
+        plan.long_len = std::max(plan.long_len, L.rd_len_cutoff);
+        if (!L.f[1].empty() || !L.f[2].empty())
+            fail("pgb200: long-read libraries (asm_flags=4) are not supported with two-file pairs (f1/f2, q1/q2); list long reads as f=, q= or p=");
+    }
+    if (has_long && plan.long_len <= 0) plan.long_len = plan.max_rd_len;
+    plan.max_len4all = std::max(plan.max_rd_len, plan.long_len);
     for (const Lib& L : libs) {
-        if (L.asm_flag == 4) fail("pgb200: long-read libraries (asm_flags=4) are not supported by the GPU map stage");
         MapLib m{L.avg_ins, L.reverse, L.map_len, L.rank, L.pair_num_cut, {}};
-        const int cut = (L.rd_len_cutoff > 0 && L.rd_len_cutoff < plan.max_rd_len) ? L.rd_len_cutoff : plan.max_rd_len;   // readseq1by1.c:1083-1090
+        const int cut = L.rd_len_cutoff > 0 ? std::min(L.rd_len_cutoff, plan.max_len4all) : plan.max_len4all;   // readseq1by1.c:1083-1090
+        if (L.asm_flag == 4) {
+            for (int type : {3, 5, 6})
+                for (const std::string& path : L.f[type]) m.files.push_back({path, type == 6, -1, L.reverse, cut});
+            plan.long_libs.push_back(m);
+            m.files.clear();
+        }
         if (L.asm_flag == 2 || L.asm_flag == 3)
             for (int type = 1; type <= 3; type++)
                 for (size_t fi = 0; fi < L.f[type].size(); fi++) {

@@ -204,6 +204,47 @@ def scenario_adversarial(d: str, seed=9, crlf=False, K_hint=31) -> str:
     return cfg
 
 
+def long_reads(g: np.ndarray, n_reads: int, min_len: int, max_len: int, seed: int, err=0.01, n_rate=0.001, short_frac=0.05,
+               K_hint=31) -> list[bytes]:
+    """Seeded long reads for a gap-closing library (asm_flags=4): lengths uniform in [min_len, max_len], both strands, i.i.d.
+    substitution errors, scattered N's, and a share `short_frac` of reads of 1..K_hint bases (shorter than K+1: they map nowhere)."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for _ in range(n_reads):
+        L = int(rng.integers(1, K_hint + 1)) if rng.random() < short_frac else int(rng.integers(min_len, max_len + 1))
+        L = min(L, len(g))
+        s = int(rng.integers(0, len(g) - L + 1))
+        r = g[s:s + L].copy()
+        if rng.random() < 0.5:
+            r = _COMP[r[::-1]]
+        r = _mutate(r, err, rng)
+        r[rng.random(L) < n_rate] = ord("N")
+        out.append(r.tobytes())
+    return out
+
+
+def write_long(path: str, reads: list[bytes], fastq: bool, tag: str = "L") -> None:
+    """Single-line FASTA or 4-line FASTQ, one record per read"""
+    with open(path, "wb") as f:
+        for i, r in enumerate(reads):
+            name = f"{tag}{i}".encode()
+            f.write(b"@" + name + b"\n" + r + b"\n+\n" + b"I" * len(r) + b"\n" if fastq else b">" + name + b"\n" + r + b"\n")
+    _pad_if_32k(path)
+
+
+def scenario_long(d: str, n_long=300, min_len=200, max_len=3000, rd_len_cutoff=5000, map_len=40, seed=21, fastq=False) -> str:
+    """scenario_pe_fastq's paired library plus one long-read library (asm_flags=4) drawn from the same genome"""
+    scenario_pe_fastq(d)
+    g = genome(60000, 3, repeat=(400, 3))   # scenario_pe_fastq's genome
+    path = os.path.join(d, "long.fq" if fastq else "long.fa")
+    write_long(path, long_reads(g, n_long, min_len, max_len, seed), fastq)
+    cfg = os.path.join(d, "long.cfg")
+    with open(cfg, "w") as f:
+        f.write(f"max_rd_len=150\n[LIB]\navg_ins=300\nreverse_seq=0\nasm_flags=3\nrank=1\nq1={d}/pe_1.fq\nq2={d}/pe_2.fq\n"
+                f"[LIB]\nasm_flags=4\nrd_len_cutoff={rd_len_cutoff}\nmap_len={map_len}\n{'q' if fastq else 'f'}={path}\n")
+    return cfg
+
+
 # ---------------------------------------------------------------- vectorised writers for the config-sized cases (millions of reads)
 def _names(n: int, tag: bytes, width: int = 9) -> np.ndarray:
     ids = np.arange(n, dtype=np.int64)
