@@ -265,6 +265,9 @@ void EngineT<NW>::build_layout() {
     }
     u64 total = 0;
     for (int i = 0; i < P; i++) { set_base[i] = total; total += set_size[i]; }
+    if (prm_.verbose)
+        fprintf(stderr, "[pgb200] layout: %llu reference slots in %d sets, %llu scan tiles\n", (unsigned long long)total, P,
+                (unsigned long long)((total + SCAN_TILE - 1) / SCAN_TILE));
     PG_CUDA(cudaMemcpyAsync(d_size, set_size.data(), P * sizeof(u64), cudaMemcpyHostToDevice, st_));
     PG_CUDA(cudaMemcpyAsync(d_base, set_base.data(), P * sizeof(u64), cudaMemcpyHostToDevice, st_));
 

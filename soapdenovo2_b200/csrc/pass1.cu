@@ -148,16 +148,29 @@ void EngineT<NW>::create_table_if_needed() {
     join_table_clear();
     if (tab_.slots) return;
     u64 want = prm_.table_slots;
-    if (!want) {
-        if (prm_.initG) {
-            // the reference's own budget: P sets of the static prime size (prlHashReads.c:369-390)
-            want = (u64)prm_.P * ref_static_set_size(prm_.initG, prm_.P, prm_.flavour127 != 0);
-            want = (want + want / 4) / (u64)(prm_.world > 1 ? prm_.world : 1);
-        } else {
-            want = 1ull << 24;
-        }
+    if (want) {
+        alloc_table(next_pow2(want < 1024 ? 1024 : want));
+        return;
     }
-    alloc_table(next_pow2(want < 1024 ? 1024 : want));
+    if (!prm_.initG) {
+        alloc_table(1ull << 24);
+        return;
+    }
+    // The reference's own budget: P sets of the static prime size (prlHashReads.c:369-390).  -a names host memory, so the same
+    // slot count can exceed HBM (-p 8 -a 21 in the 63-mer build asks for 2^31 slots, 64 GiB).  The table grows on demand, so it
+    // starts at the largest power of two that leaves room for the layout's reference-order buffer (8 B per reference slot) and its
+    // 8 B per table slot, with a quarter of the free HBM kept for the exchange arena and the reads.
+    const u64 ref_slots = (u64)prm_.P * ref_static_set_size(prm_.initG, prm_.P, prm_.flavour127 != 0);
+    want = (ref_slots + ref_slots / 4) / (u64)(prm_.world > 1 ? prm_.world : 1);
+    u64 cap = next_pow2(want < 1024 ? 1024 : want);
+    size_t free_b = 0, total_b = 0;
+    PG_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const u64 budget = (u64)free_b / 4 * 3, fixed = ref_slots * sizeof(u64) + (1ull << 30);
+    while (cap > (1ull << 24) && cap * (sizeof(Slot<NW>) + sizeof(u64)) + fixed > budget) cap >>= 1;
+    if (prm_.verbose && cap < next_pow2(want))
+        fprintf(stderr, "[pgb200] k-mer table starts at %llu slots (the -a budget asks for %llu; the rest of HBM is kept for the layout)\n",
+                (unsigned long long)cap, (unsigned long long)next_pow2(want));
+    alloc_table(cap);
 }
 
 // Inserts whose new keys are bounded from above keep the table under TABLE_LOAD; when HBM allows no growth, it may fill up to

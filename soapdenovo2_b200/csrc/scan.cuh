@@ -121,7 +121,8 @@ void device_scan(In in, Out out, u64 n, u64* scratch, u64* d_total, cudaStream_t
     if (tiles <= (u64)SCAN_TILE * 64) {
         k_scan_small<<<1, SCAN_THREADS, 0, st>>>(sums, tiles, d_total);
     } else {
-        // second level (only for > 1e9-element inputs)
+        // second level: more than 4096 x 262144 elements.  The layout scans the reference's set geometry, which -a sizes from the
+        // memory the user names, so any -a large enough reaches it (-p 8 -a 21 in the 63-mer build)
         u64* sums2 = scratch + tiles + 1;
         device_scan(ScanU64In{sums}, ScanU64Out{sums}, tiles, sums2, d_total, st);
     }

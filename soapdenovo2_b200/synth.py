@@ -223,6 +223,29 @@ def long_reads(g: np.ndarray, n_reads: int, min_len: int, max_len: int, seed: in
     return out
 
 
+def long_reads_of_lengths(g: np.ndarray, lengths: list[int], seed: int, err=0.01, n_rate=0.001) -> list[bytes]:
+    """long_reads() with the read lengths given: one read per length, drawn as long_reads() draws them"""
+    rng = np.random.default_rng(seed)
+    out = []
+    for L in lengths:
+        s = int(rng.integers(0, len(g) - L + 1))
+        r = g[s:s + L].copy()
+        if rng.random() < 0.5:
+            r = _COMP[r[::-1]]
+        r = _mutate(r, err, rng)
+        r[rng.random(L) < n_rate] = ord("N")
+        out.append(r.tobytes())
+    return out
+
+
+def tiled_pairs(g: np.ndarray, step: int, rd_len: int, insert: int) -> tuple[np.ndarray, np.ndarray]:
+    """Error-free pairs at every `step`-th genome position: pair i has mate 1 = g[s:s+rd_len] and mate 2 = the reverse complement of
+    g[s+insert-rd_len:s+insert], s = i*step, for every s <= len(g) - insert (so every base is covered when step <= rd_len)."""
+    starts = np.arange(0, len(g) - insert + 1, step, dtype=np.int64)
+    win = np.lib.stride_tricks.sliding_window_view(g, rd_len)   # no per-base index array (millions of reads)
+    return win[starts], _revcomp(win[starts + insert - rd_len])
+
+
 def write_long(path: str, reads: list[bytes], fastq: bool, tag: str = "L") -> None:
     """Single-line FASTA or 4-line FASTQ, one record per read"""
     with open(path, "wb") as f:
