@@ -72,8 +72,9 @@ struct ReadChunk {
 };
 
 enum Counter { C_DISTINCT = 0, C_INSTANCES, C_KEPT, C_LINEAR, C_REMOVED, C_MISC0, C_MISC1, C_MISC2, C_BADFMT, C_XERR, C_XUSED, C_RESERVED, C_DEFER, C_MAXU,
-               C_XSEGS, C_XEPOCH, C_SPILLKEYS, C_REDO, C_COUNT };   // C_SPILLKEYS: keys the aggregation stored WITHOUT the fused sweeps;
-                                                                 // C_REDO: records decoded by the general rules (k_decode_fix)
+               C_XSEGS, C_XEPOCH, C_SPILLKEYS, C_REDO, C_SKM_STAGED, C_SKM_DRAINED, C_COUNT };
+               // C_SPILLKEYS: keys the aggregation stored WITHOUT the fused sweeps; C_REDO: records decoded by the general rules (k_decode_fix);
+               // C_SKM_STAGED / C_SKM_DRAINED: records an aggregation read, distinct records it expanded (k_skm_apply)
 
 // What an aggregation launch reports: C_XERR .. C_MAXU, read with one copy
 struct FlushOutcome { u64 xerr, xused, reserved, defer, maxu; };

@@ -25,9 +25,11 @@ namespace pgb {
 
 constexpr int SKM_PART_THREADS = 128;
 constexpr int SKM_APPLY_THREADS = 256;
-// Shared-memory table of a bucket: 1024 slots (32 KB at K <= 63) plus the record stage (SKM_STAGE_RECS) put 4 CTAs = 32 warps on an
-// H100 SM (4 x 47 KB of 228 KB) at 64 registers per thread; 256-bit keys (48 B slots, 69 KB per CTA) run 3 CTAs.  On H100 this beat
-// 3 CTAs with a 256-record stage and 4 with a 192-record one (DESIGN.md §5); 5 or 6 CTAs spill at the register budget they allow.
+// Shared-memory table of a bucket: 1024 slots (32 KB at K <= 63) plus the record stage (2 x SKM_STAGE_RECS = 64 records), the
+// distinct-record buffer (SKM_BUF_RECS = 128 records, their reversed bases, counts and dedup table) put 4 CTAs = 32 warps on an H100
+// SM (4 x 48 KB of 228 KB) at 64 registers per thread; 256-bit keys (48 B slots, 71 KB per CTA) run 3 CTAs at 72 registers.  No stack
+// frame and no spills at either width.  The stage was 2 x 128 records before the buffer existed; halving it pays for the buffer at
+// K > 63.  5 or 6 CTAs spill at the register budget they allow.
 #ifndef SKM_LOG2_SLOTS
 #define SKM_LOG2_SLOTS 10
 #endif
@@ -289,12 +291,13 @@ struct SmemTable {
         }
         return 3;
     }
-    __device__ __forceinline__ void apply(u32 idx, unsigned left, unsigned right, u64 rank) const {
+    // c identical instances
+    __device__ __forceinline__ void apply(u32 idx, unsigned left, unsigned right, u64 rank, unsigned c) const {
         volatile u64* vpay = pay;
         volatile u64* vrnk = rnk;
         u64 cur = vpay[idx];
         for (;;) {
-            u64 nxt = payload_apply(cur, left, right);
+            u64 nxt = payload_apply_n(cur, left, right, c);
             if (nxt == cur) break;
             u64 old = atomicCAS(&pay[idx], cur, nxt);
             if (old == cur) break;
@@ -379,9 +382,10 @@ struct SkmApplyArgs {
 constexpr u64 SKM_CREDIT = 1ull << 16;   // table room a CTA reserves at a time (keys)
 
 // -DSKM_PHASE_CLOCKS: k_skm_apply adds up clock64() per phase over all its threads (stage wait, instance build, find / claim, apply,
-// spill to the global table, flush); the host prints the totals of every aggregation with PGB200_SKM_STATS.  Off: no code at all.
+// spill to the global table, flush, record dedup); the host prints the totals of every aggregation with PGB200_SKM_STATS.  Off: no
+// code at all.
 #ifdef SKM_PHASE_CLOCKS
-constexpr int SKM_PHASES = 6;
+constexpr int SKM_PHASES = 7;
 __device__ unsigned long long g_skm_phase_clk[SKM_PHASES];
 #define SKM_T0(v) const long long v = clock64()
 #define SKM_ACC(i, v) clk[i] += (u64)(clock64() - (v))
@@ -414,12 +418,59 @@ __device__ __forceinline__ u32 cta_exclusive_scan(u32 v, u32* s_warp, u32& total
 
 // Records of one bucket staged per window: the window is W consecutive records of the bucket's concatenated segment ranges; every
 // segment thread copies its part of the window with one bulk copy, completed on the half's mbarrier.  The stage is double-buffered:
-// the next window (or the next bucket's first) is in flight while the current one is processed, flushed and synchronised.
+// the next window (or the next bucket's first) is in flight while the current one is processed and synchronised.  A window is only
+// collapsed into the distinct-record buffer (skm_dedup_insert), so the stage just has to keep the bulk copies ahead.
 #ifndef SKM_STAGE_RECS
-#define SKM_STAGE_RECS 128
+#define SKM_STAGE_RECS 64
 #endif
 constexpr int SKM_W = SKM_STAGE_RECS;
-static_assert(SKM_W <= SKM_APPLY_THREADS, "the per-record pre-pass runs one thread per staged record");
+constexpr int SKM_BUF_RECS = 128;        // distinct records buffered before they are expanded into k-mer instances (a drain)
+constexpr int SKM_DEDUP_SLOTS = 256;     // the buffer's hash table: record -> buffer position
+static_assert(SKM_W <= SKM_BUF_RECS && SKM_BUF_RECS <= SKM_APPLY_THREADS, "one drain empties the buffer for a whole window; one thread per buffered record");
+static_assert(SKM_BUF_RECS + SKM_W < SKM_DEDUP_SLOTS && (SKM_DEDUP_SLOTS & (SKM_DEDUP_SLOTS - 1)) == 0, "the dedup table never fills up");
+
+constexpr u32 SKM_DD_EMPTY = 0xFFFFFFFFu, SKM_DD_BUSY = 0xFFFFFFFEu, SKM_DD_FULL = 0xFFFFFFFDu;
+// One staged record r into the distinct-record buffer: find-or-claim its entry in the dedup table (claim: CAS EMPTY -> BUSY, take
+// a buffer position, copy the record with count 1, fence, publish the position); a copy adds 1 to the count and lowers the buffered
+// header to the smaller of the two (skm_rec_same).  Returns true when the record found no room (the claim came after the buffer's
+// SKM_BUF_RECS positions were taken, or the probe met such a claim, marked FULL): the caller drains the buffer and calls again.
+template <int NW>
+__device__ __forceinline__ bool skm_dedup_insert(const u64* r, u64* buf, u32* cnt, u32* dd, u32* nbuf) {
+    constexpr int RW = NW + 2;
+    volatile u32* vdd = dd;
+    u32 idx = skm_rec_hash<NW>(r) >> (32 - __builtin_ctz(SKM_DEDUP_SLOTS));
+    for (;;) {
+        u32 v = vdd[idx];
+        if (v == SKM_DD_EMPTY) {
+            v = atomicCAS(&dd[idx], SKM_DD_EMPTY, SKM_DD_BUSY);
+            if (v == SKM_DD_EMPTY) {
+                const u32 j = atomicAdd(nbuf, 1u);
+                if (j >= (u32)SKM_BUF_RECS) {
+                    vdd[idx] = SKM_DD_FULL;
+                    return true;
+                }
+#pragma unroll
+                for (int i = 0; i < RW; i++) buf[j * RW + i] = r[i];
+                cnt[j] = 1;
+                __threadfence_block();
+                vdd[idx] = j;
+                return false;
+            }
+        }
+        while (v == SKM_DD_BUSY) v = vdd[idx];
+        if (v == SKM_DD_FULL) return true;
+        u64 b[RW];
+        const volatile u64* vb = buf + v * RW;
+#pragma unroll
+        for (int i = 0; i < RW; i++) b[i] = vb[i];
+        if (skm_rec_same<NW>(b, r)) {
+            atomicAdd(&cnt[v], 1u);
+            atomicMin((unsigned long long*)&buf[v * RW], (unsigned long long)r[0]);
+            return false;
+        }
+        idx = (idx + 1) & (SKM_DEDUP_SLOTS - 1);
+    }
+}
 
 // A segment thread's part of one bucket: records lo .. lo+cnt-1 of its segment, at positions cum .. cum+cnt-1 of the bucket.
 struct SkmSegRange {
@@ -442,23 +493,30 @@ __device__ __forceinline__ void skm_stage_window(u64* stage, u64* bar, const u64
 
 // One CTA per bucket (static round-robin over the list: buckets are hash-uniform), one shared-memory table per CTA.  A bucket is
 // processed window by window (skm_stage_window); the table persists over the windows and is flushed once per bucket.  When a window
-// has landed, one thread per record writes its k-mer count prefix P and its reversed bases (skm_rec_reverse) next to the stage.  The
-// warps then split the window's instances into contiguous slices and take 32 CONSECUTIVE instances per step -- all lanes busy
-// whatever the run lengths: the records that start inside the step come from one lookahead load of P, and every lane builds its
-// k-mer and reverse complement with two shifts of shared-memory words (skm_instance_staged).
+// has landed, one thread per record collapses it into the buffer of distinct records (skm_dedup_insert): at 30x most records of a
+// bucket are copies of another one.  The buffer is drained into the table when it is full and at the end of the bucket: one thread
+// per buffered record writes its k-mer count prefix P and its reversed bases (skm_rec_reverse), then the warps split the buffer's
+// instances into contiguous slices and take 32 CONSECUTIVE instances per step -- all lanes busy whatever the run lengths: the
+// records that start inside the step come from one lookahead load of P, and every lane builds its k-mer and reverse complement with
+// two shifts of shared-memory words (skm_instance_staged) and applies it as many times as its record occurred.
 template <int NW>
 __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k_skm_apply(Table<NW> tab, KParams<NW> kp, SkmApplyArgs a) {
-    constexpr int RW = NW + 2, WARPS = SKM_APPLY_THREADS / 32;
-    // key[NW][S], pay[S], rnk[S], stage[2][W][RW], rv[W][NW+1], list[S] (u16), P[W+1]
+    constexpr int RW = NW + 2, WARPS = SKM_APPLY_THREADS / 32, C = SKM_BUF_RECS;
+    // key[NW][S], pay[S], rnk[S], stage[2][W][RW], buf[C][RW], rv[C][NW+1], list[S] (u16), P[C+1], cnt[C], dedup[DS]
     extern __shared__ __align__(16) u64 s_dyn[];
     u64* const s_stage = s_dyn + (NW + 2) * SKM_SLOTS;
-    u64* const s_rv = s_stage + 2 * SKM_W * RW;
-    unsigned short* const s_list = reinterpret_cast<unsigned short*>(s_rv + SKM_W * (NW + 1));
+    u64* const s_buf = s_stage + 2 * SKM_W * RW;
+    u64* const s_rv = s_buf + C * RW;
+    unsigned short* const s_list = reinterpret_cast<unsigned short*>(s_rv + C * (NW + 1));
     u32* const s_P = reinterpret_cast<u32*>(s_list + SKM_SLOTS);
+    u32* const s_cnt = s_P + C + 1;
+    u32* const s_dd = s_cnt + C;
     __shared__ __align__(8) u64 s_bar[2];
     __shared__ u32 s_warp[WARPS];
-    __shared__ u32 s_count, s_defer;
+    __shared__ u32 s_count, s_defer, s_nbuf;
+    __shared__ unsigned char s_pend[SKM_W];   // the window's records still to be collapsed into the buffer
     __shared__ unsigned s_new, s_tot_new;
+    __shared__ u64 s_staged, s_drained;   // records staged, distinct records drained (PGB200_SKM_STATS)
     __shared__ SweepTally s_sw;   // the fused sweeps (a.sweep)
     SmemTable<NW, SKM_SLOTS, SKM_SOFT_LIMIT, unsigned short> st{s_dyn, s_dyn + NW * SKM_SLOTS, s_dyn + (NW + 1) * SKM_SLOTS, s_list, &s_count};
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -468,8 +526,12 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         st.pay[i] = PAYLOAD_FRESH;
         st.rnk[i] = ~0ull;
     }
+    for (int i = tid; i < SKM_DEDUP_SLOTS; i += SKM_APPLY_THREADS) s_dd[i] = SKM_DD_EMPTY;   // each drain re-empties it
     if (tid == 0) {
         s_tot_new = 0;
+        s_nbuf = 0;
+        s_staged = 0;
+        s_drained = 0;
         mbar_init(&s_bar[0], 1);
         mbar_init(&s_bar[1], 1);
     }
@@ -479,8 +541,9 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     const int n_segs = (int)a.segs->n;
     const u32* my_so = tid < n_segs ? a.segs->segoff[tid] : nullptr;
     const u64* my_recs = tid < n_segs ? a.segs->recs[tid] : nullptr;
-    unsigned tot_new = 0;
-    u64 credit = 0;                      // thread 0: table room this CTA holds
+    __shared__ u64 s_credit;             // thread 0: table room this CTA holds (not in a register: the drain needs them all)
+    u64& credit = s_credit;
+    if (tid == 0) credit = 0;
 #ifdef SKM_PHASE_CLOCKS
     u64 clk[SKM_PHASES] = {};
 #endif
@@ -538,7 +601,84 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         }
         __syncthreads();
         const bool run = !s_defer && R > 0;
-        unsigned my_new = 0;
+        // ---- drain: the nb buffered records -> their k-mer instances -> the shared-memory table; the buffer is empty again
+        auto drain = [&](u32 nb) {
+            SKM_T0(t_pre);
+            // per record: its k-mer count prefix and its reversed bases
+            u32 n = 0;
+            if ((u32)tid < nb) {
+                const u64 hdr = s_buf[tid * RW];
+                n = (u32)skm_rec_n(hdr);
+                u64 rv[NW + 1];
+                skm_rec_reverse<NW>(hdr, s_buf + tid * RW + 1, rv, kp.K);
+#pragma unroll
+                for (int i = 0; i < NW + 1; i++) s_rv[tid * (NW + 1) + i] = rv[i];
+            }
+            u32 I;
+            const u32 p = cta_exclusive_scan(n, s_warp, I);
+            if ((u32)tid < nb) s_P[tid] = p;
+            if (tid == 0) s_P[nb] = I;
+            __syncthreads();
+            SKM_ACC(1, t_pre);
+            // ---- the warps: contiguous slices of the buffer's instances, 32 consecutive instances per step
+            const u32 steps = (I + 31) / 32, per = (steps + WARPS - 1) / WARPS;
+            const u32 q_end = min(I, (wid + 1) * per * 32);
+            u32 q0 = wid * per * 32;
+            u32 r0 = 0;   // the record holding q0: the last record with P <= q0
+            if (q0 < q_end) {
+                u32 lo = 0, hi = nb;
+                while (hi - lo > 1) {
+                    const u32 mid = (lo + hi) >> 1;
+                    if (s_P[mid] <= q0) lo = mid; else hi = mid;
+                }
+                r0 = lo;
+            }
+            for (; q0 < q_end; q0 += 32) {
+                const u32 q = q0 + lane;
+                const bool has = q < q_end;
+                SKM_T0(t_inst);
+                // the records that start at step positions 1 .. 31 (P is strictly increasing: every record holds a k-mer)
+                const u32 pn = s_P[min(r0 + 1 + lane, nb)];
+                const unsigned starts = __reduce_or_sync(0xffffffffu, pn - q0 - 1 < 31u ? 1u << (pn - q0) : 0u);
+                const u32 rec = r0 + __popc(starts & lane_le);
+                r0 += __popc(__ballot_sync(0xffffffffu, pn <= q0 + 32));
+                const unsigned has_mask = __ballot_sync(0xffffffffu, has);
+                if (has) {
+                    const int t = (int)(q - s_P[rec]);
+                    const u64 h = s_buf[rec * RW];
+                    const unsigned c = s_cnt[rec];
+                    const SkmInst<NW> in = skm_instance_staged<NW>(kp, h, s_buf + rec * RW + 1, s_rv + rec * (NW + 1), t);
+                    const u64 rank = skm_rec_rank(h, t);
+                    SKM_ACC(1, t_inst);
+                    SKM_T0(t_find);
+                    u32 slot;
+                    const int state = st.find(tab, in.canon, slot);
+                    __syncwarp(has_mask);   // the lanes re-join before the counter update (see SmemTable)
+                    SKM_ACC(2, t_find);
+                    SKM_T0(t_upd);
+                    if (state == 1) {
+                        st.apply(slot, in.left, in.right, rank, c);
+                        SKM_ACC(3, t_upd);
+                    } else if (state == 3) {
+                        // bucket holds more distinct k-mers than the shared-memory table: this k-mer goes to HBM directly (same result;
+                        // the CAS protocol, since lanes may spill the same new key at once)
+                        u64 at;
+                        const bool fresh = table_insert(tab, in.canon, in.left, in.right, rank, &at, c);
+                        if (fresh) atomicAdd(&s_new, 1u);
+                        if (fresh && a.sweep) {   // its other instances follow the same way: swept after the launch, from this list
+                            const u64 sn = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
+                            if (sn < a.spill_cap) a.spill_list[sn] = at;
+                        }
+                        SKM_ACC(4, t_upd);
+                    }
+                }
+                __syncwarp();
+            }
+            __syncthreads();   // the buffer, its counts, P and rv are free again
+            for (int i = tid; i < SKM_DEDUP_SLOTS; i += SKM_APPLY_THREADS) s_dd[i] = SKM_DD_EMPTY;
+            if (tid == 0) { s_nbuf = 0; s_drained += nb; }
+            __syncthreads();
+        };
         // ---- the windows of the bucket (a deferred or empty bucket still retires the window queued for it)
         for (u32 w = 0;; w++) {
             const bool more = run && (w + 1) * (u32)SKM_W < R;
@@ -549,79 +689,23 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             SKM_ACC(0, t_wait);
             phase ^= 1u << half;
             if (run) {
-                SKM_T0(t_pre);
                 const u64* stg = s_stage + half * SKM_W * RW;
                 const u32 nrec = min(R - w * (u32)SKM_W, (u32)SKM_W);
-                // per record: its k-mer count prefix and its reversed bases
-                u32 n = 0;
-                if ((u32)tid < nrec) {
-                    const u64 hdr = stg[tid * RW];
-                    n = (u32)skm_rec_n(hdr);
-                    u64 rv[NW + 1];
-                    skm_rec_reverse<NW>(hdr, stg + tid * RW + 1, rv, kp.K);
-#pragma unroll
-                    for (int i = 0; i < NW + 1; i++) s_rv[tid * (NW + 1) + i] = rv[i];
-                }
-                u32 I;
-                const u32 p = cta_exclusive_scan(n, s_warp, I);
-                if ((u32)tid < nrec) s_P[tid] = p;
-                if (tid == 0) s_P[nrec] = I;
-                __syncthreads();
-                SKM_ACC(1, t_pre);
-                // ---- the warps: contiguous slices of the window's instances, 32 consecutive instances per step
-                const u32 steps = (I + 31) / 32, per = (steps + WARPS - 1) / WARPS;
-                const u32 q_end = min(I, (wid + 1) * per * 32);
-                u32 q0 = wid * per * 32;
-                u32 r0 = 0;   // the record holding q0: the last record with P <= q0
-                if (q0 < q_end) {
-                    u32 lo = 0, hi = nrec;
-                    while (hi - lo > 1) {
-                        const u32 mid = (lo + hi) >> 1;
-                        if (s_P[mid] <= q0) lo = mid; else hi = mid;
-                    }
-                    r0 = lo;
-                }
-                for (; q0 < q_end; q0 += 32) {
-                    const u32 q = q0 + lane;
-                    const bool has = q < q_end;
-                    SKM_T0(t_inst);
-                    // the records that start at step positions 1 .. 31 (P is strictly increasing: every record holds a k-mer)
-                    const u32 pn = s_P[min(r0 + 1 + lane, nrec)];
-                    const unsigned starts = __reduce_or_sync(0xffffffffu, pn - q0 - 1 < 31u ? 1u << (pn - q0) : 0u);
-                    const u32 rec = r0 + __popc(starts & lane_le);
-                    r0 += __popc(__ballot_sync(0xffffffffu, pn <= q0 + 32));
-                    const unsigned has_mask = __ballot_sync(0xffffffffu, has);
-                    if (has) {
-                        const int t = (int)(q - s_P[rec]);
-                        const u64 h = stg[rec * RW];
-                        const SkmInst<NW> in = skm_instance_staged<NW>(kp, h, stg + rec * RW + 1, s_rv + rec * (NW + 1), t);
-                        const u64 rank = skm_rec_rank(h, t);
-                        SKM_ACC(1, t_inst);
-                        SKM_T0(t_find);
-                        u32 slot;
-                        const int state = st.find(tab, in.canon, slot);
-                        __syncwarp(has_mask);   // the lanes re-join before the counter update (see SmemTable)
-                        SKM_ACC(2, t_find);
-                        SKM_T0(t_upd);
-                        if (state == 1) {
-                            st.apply(slot, in.left, in.right, rank);
-                            SKM_ACC(3, t_upd);
-                        } else if (state == 3) {
-                            // bucket holds more distinct k-mers than the shared-memory table: this instance goes to HBM directly (same result)
-                            u64 at;
-                            const bool fresh = table_insert(tab, in.canon, in.left, in.right, rank, &at);
-                            my_new += fresh;
-                            if (fresh && a.sweep) {   // its other instances follow the same way: swept after the launch, from this list
-                                const u64 sn = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
-                                if (sn < a.spill_cap) a.spill_list[sn] = at;
-                            }
-                            SKM_ACC(4, t_upd);
-                        }
-                    }
-                    __syncwarp();
+                if (tid == 0) s_staged += nrec;
+                if (tid < SKM_W) s_pend[tid] = (u32)tid < nrec;   // (in shared memory: nothing of the window stays in registers over a drain)
+                for (;;) {
+                    SKM_T0(t_dd);
+                    if (tid < SKM_W && s_pend[tid]) s_pend[tid] = skm_dedup_insert<NW>(stg + tid * RW, s_buf, s_cnt, s_dd, &s_nbuf);
+                    __syncthreads();
+                    SKM_ACC(6, t_dd);
+                    const u32 nb = s_nbuf;
+                    const bool full = nb > (u32)C;
+                    if (!full && (more || nb == 0)) break;
+                    drain(min(nb, (u32)C));   // full (the records that found no room go into the emptied buffer), or the bucket's end
+                    if (!full) break;
                 }
             }
-            __syncthreads();   // the window's stage half, P and rv are free again
+            __syncthreads();   // the window's stage half is free again
             half ^= 1;
             if (!more) break;
         }
@@ -632,6 +716,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         // ---- flush: one global update per distinct k-mer of the bucket, walking the claim list (every thread busy)
         SKM_T0(t_flush);
         const u32 n_claimed = s_count;
+        unsigned my_new = 0;
         for (u32 i = tid; i < n_claimed; i += SKM_APPLY_THREADS) {
             const u32 idx = st.list[i];
             Kmer<NW> k;
@@ -647,16 +732,21 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             st.rnk[idx] = ~0ull;
         }
         if (my_new) atomicAdd(&s_new, my_new);
-        tot_new += my_new;
         __syncthreads();
         SKM_ACC(5, t_flush);
-        if (tid == 0) credit += (u64)R * SKM_MAX_RUN - (u64)s_new;   // what the bound over-reserved stays with the CTA
+        if (tid == 0) {
+            credit += (u64)R * SKM_MAX_RUN - (u64)s_new;   // what the bound over-reserved stays with the CTA
+            s_tot_new += s_new;
+        }
     }
     __syncthreads();
     if (tid == 0 && credit) atomicAdd((unsigned long long*)&a.counters[C_RESERVED], (unsigned long long)(0ull - credit));
-    if (tot_new) atomicAdd(&s_tot_new, tot_new);
     s_sw.flush(sw_lin, sw_rem, a.hist, &a.counters[C_LINEAR], &a.counters[C_REMOVED]);   // (all zero without a.sweep)
     if (tid == 0 && s_tot_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_tot_new);
+    if (tid == 0 && s_staged) {
+        atomicAdd(&a.counters[C_SKM_STAGED], s_staged);
+        atomicAdd(&a.counters[C_SKM_DRAINED], s_drained);
+    }
 #ifdef SKM_PHASE_CLOCKS
     for (int i = 0; i < SKM_PHASES; i++) atomicAdd(&g_skm_phase_clk[i], (unsigned long long)clk[i]);
 #endif
@@ -665,8 +755,8 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
 // ------------------------------------------------------------------------------------------------ host side
 template <int NW>
 static constexpr size_t skm_apply_smem() {
-    return ((size_t)(NW + 2) * SKM_SLOTS + 2 * SKM_W * (NW + 2) + SKM_W * (NW + 1)) * sizeof(u64) + (size_t)SKM_SLOTS * sizeof(unsigned short) +
-           (SKM_W + 1) * sizeof(u32);
+    return ((size_t)(NW + 2) * SKM_SLOTS + 2 * SKM_W * (NW + 2) + SKM_BUF_RECS * (NW + 2) + SKM_BUF_RECS * (NW + 1)) * sizeof(u64) +
+           (size_t)SKM_SLOTS * sizeof(unsigned short) + (2 * SKM_BUF_RECS + 1 + SKM_DEDUP_SLOTS) * sizeof(u32);
 }
 // An aggregation launch keeps the keys the table is committed to under this share of its capacity (buckets beyond it are deferred),
 // and the growth before their re-run leaves this much HBM free
@@ -989,6 +1079,7 @@ void EngineT<NW>::skm_flush(bool final_of_pass) {
         PG_CUDA(cudaMemsetAsync(d_cnt_ + C_LINEAR, 0, 2 * sizeof(u64), st_));
     }
     pass_sweeps_ = flush_.sweep ? PassSweeps::Fused : PassSweeps::Plain;
+    PG_CUDA(cudaMemsetAsync(d_cnt_ + C_SKM_STAGED, 0, 2 * sizeof(u64), st_));
     flush_.half = (int)(xa_flushed_epoch_ % SKM_ARENA_HALVES);
     PG_CUDA(cudaEventRecord(ev_flush_begin_, st_));
     skm_launch_apply(nullptr, skm_own_hi_ - skm_own_lo_, skm_deferred_[0].template as<u32>());
@@ -1028,9 +1119,13 @@ void EngineT<NW>::skm_flush_complete() {
     p1_.ms_insert += ms;
     p1_.ms_apply += ms;
     xa_flushed_epoch_++;
-    if (prm_.verbose >= 2 || getenv("PGB200_SKM_STATS"))
-        fprintf(stderr, "[pgb200] aggregated epoch %llu: %u owned bucket(s), %d launch(es), %.2f ms, table %llu slots\n", (unsigned long long)xa_flushed_epoch_,
-                skm_own_hi_ - skm_own_lo_, launches, ms, (unsigned long long)cap_);
+    if (prm_.verbose >= 2 || getenv("PGB200_SKM_STATS")) {
+        u64 rd[2];   // C_SKM_STAGED, C_SKM_DRAINED
+        PG_CUDA(cudaMemcpy(rd, d_cnt_ + C_SKM_STAGED, sizeof(rd), cudaMemcpyDeviceToHost));
+        fprintf(stderr, "[pgb200] aggregated epoch %llu: %u owned bucket(s), %d launch(es), %.2f ms, table %llu slots, %llu records staged, %llu distinct "
+                        "drained (%.3f)\n", (unsigned long long)xa_flushed_epoch_, skm_own_hi_ - skm_own_lo_, launches, ms, (unsigned long long)cap_,
+                (unsigned long long)rd[0], (unsigned long long)rd[1], rd[0] ? (double)rd[1] / (double)rd[0] : 0.0);
+    }
 #ifdef SKM_PHASE_CLOCKS
     if (getenv("PGB200_SKM_STATS")) {
         unsigned long long c[SKM_PHASES], zero[SKM_PHASES] = {}, tot = 0;
@@ -1038,8 +1133,8 @@ void EngineT<NW>::skm_flush_complete() {
         PG_CUDA(cudaMemcpyToSymbol(g_skm_phase_clk, zero, sizeof(zero)));
         for (int i = 0; i < SKM_PHASES; i++) tot += c[i];
         fprintf(stderr, "[pgb200] aggregation phase clocks (thread-cycles, %% of %.3g): stage wait %.1f, instance build %.1f, find/claim %.1f, apply %.1f, "
-                        "spill %.1f, flush %.1f\n", (double)tot, 100.0 * c[0] / tot, 100.0 * c[1] / tot, 100.0 * c[2] / tot, 100.0 * c[3] / tot, 100.0 * c[4] / tot,
-                100.0 * c[5] / tot);
+                        "spill %.1f, flush %.1f, dedup %.1f\n", (double)tot, 100.0 * c[0] / tot, 100.0 * c[1] / tot, 100.0 * c[2] / tot, 100.0 * c[3] / tot,
+                100.0 * c[4] / tot, 100.0 * c[5] / tot, 100.0 * c[6] / tot);
     }
 #endif
 }

@@ -425,6 +425,31 @@ PG_HD SkmInst<NW> skm_instance_staged(const KParams<NW>& kp, u64 hdr, const u64*
     return r;
 }
 
+// ---------------------------------------------------------------- collapsing repeated records
+// Two records with equal header bits 0-7 (n, last, has_prev) and equal base words make the same k-mer instances (skm_make_rec zeroes
+// every base past the meaningful ones): only the ranks differ.  Copy r's k-mer t has rank (ord_r << 16) | (start_r + t), so the
+// smallest rank over the copies is that of the copy with the smallest header (the low 8 bits being equal, headers order by
+// (ordinal, start)).  The aggregation (skm.cu) therefore keeps each distinct record once, with the minimum header and a count c,
+// and applies its k-mers with payload_apply_n(.., c): the same {payload, rank} per k-mer as every copy expanded on its own.
+template <int NW>
+PG_HD bool skm_rec_same(const u64* a, const u64* b) {
+    bool same = ((a[0] ^ b[0]) & 0xFF) == 0;
+#pragma unroll
+    for (int i = 1; i < NW + 2; i++) same = same && a[i] == b[i];
+    return same;
+}
+// hash of the part skm_rec_same compares
+template <int NW>
+PG_HD u32 skm_rec_hash(const u64* r) {
+    u64 x = r[0] & 0xFF;
+#pragma unroll
+    for (int i = 1; i < NW + 2; i++) {
+        x = (x ^ r[i]) * 0x9E3779B97F4A7C15ull;
+        x ^= x >> 29;
+    }
+    return (u32)(x >> 32);
+}
+
 // ---------------------------------------------------------------- lane packing
 // P[0..nt] = exclusive prefix sums of the k-mer counts of a tile of nt records.  Instance q of the tile belongs to the last record r
 // with P[r] <= q (every record holds at least one k-mer, so P is strictly increasing); its position inside the record is q - P[r].

@@ -61,6 +61,28 @@ PG_HD u64 payload_apply(u64 p, unsigned left, unsigned right) {
     if ((il | ir) != 0ull && (p & mc) != mc) inc |= 1ull << PL_COV_SHIFT;
     return (p + inc) & ~PL_SINGLE;
 }
+// c identical instances applied at once: equals c calls of payload_apply (c >= 1), and IS payload_apply when c == 1.  The aggregation
+// applies each k-mer of a record that occurs c times in its bucket this way (skm.cu).
+PG_HD u64 payload_apply_n(u64 p, unsigned left, unsigned right, unsigned c) {
+    if (c == 1) return payload_apply(p, left, right);
+    if (p == PAYLOAD_FRESH) { p = payload_apply(p, left, right); c--; }
+    c = c > 255 ? 255u : c;
+    if (left < 4) {
+        const int sh = 6 * (int)left;
+        const unsigned v = (unsigned)((p >> sh) & 63) + c;
+        p = (p & ~(63ull << sh)) | ((u64)(v > 63 ? 63 : v) << sh);
+    }
+    if (right < 4) {
+        const int sh = PL_R_SHIFT + 6 * (int)right;
+        const unsigned v = (unsigned)((p >> sh) & 63) + c;
+        p = (p & ~(63ull << sh)) | ((u64)(v > 63 ? 63 : v) << sh);
+    }
+    if (left < 4 || right < 4) {
+        const unsigned v = pl_cov(p) + c;
+        p = (p & ~(255ull << PL_COV_SHIFT)) | ((u64)(v > 255 ? 255 : v) << PL_COV_SHIFT);
+    }
+    return p & ~PL_SINGLE;
+}
 
 // The per-entry sweeps of pass 1's end (K4): delow (thread_delow: zero every link counter <= D, deleted = 1 if nothing is left), mark
 // (thread_mark: linear = 1 iff exactly one non-zero left and one non-zero right link, NO deleted check there), histogram of cov.
@@ -236,10 +258,11 @@ PG_D u64 table_find(const Table<NW>& t, const Kmer<NW>& k) {
 // slot's {payload, aux} words (per-instance insert, aggregated merge, spills) uses these same two 64-bit atomics: atomics of
 // different widths on overlapping words are not guaranteed to be atomic with respect to each other.
 // Order-independent: the final {payload, rank} is a pure function of the multiset of instances (SURVEY.md A.3).
+// c > 1: c identical instances (payload_apply_n).
 template <int NW>
-PG_D void slot_apply(Slot<NW>* s, u64 cur_payload, u64 cur_rank, unsigned left, unsigned right, u64 rank) {
+PG_D void slot_apply(Slot<NW>* s, u64 cur_payload, u64 cur_rank, unsigned left, unsigned right, u64 rank, unsigned c = 1) {
     for (;;) {
-        u64 nxt = payload_apply(cur_payload, left, right);
+        u64 nxt = payload_apply_n(cur_payload, left, right, c);
         if (nxt == cur_payload) break;                       // saturated: read-only
         u64 old = atomicCAS(&s->payload, cur_payload, nxt);
         if (old == cur_payload) break;
@@ -248,21 +271,21 @@ PG_D void slot_apply(Slot<NW>* s, u64 cur_payload, u64 cur_rank, unsigned left, 
     if (rank < cur_rank) atomicMin(&s->aux, rank);
 }
 
-// Fused find-or-claim + apply for one k-mer instance.  Returns true if this call inserted the key.
+// Fused find-or-claim + apply for one k-mer instance (c identical instances).  Returns true if this call inserted the key.
 template <int NW>
-PG_D bool table_insert(const Table<NW>& t, const Kmer<NW>& k, unsigned left, unsigned right, u64 rank, u64* idx_out = nullptr) {
+PG_D bool table_insert(const Table<NW>& t, const Kmer<NW>& k, unsigned left, unsigned right, u64 rank, u64* idx_out = nullptr, unsigned c = 1) {
     bool claimed;
     u64 idx = table_find_or_claim(t, k, &claimed);
     if (idx_out) *idx_out = idx;
     Slot<NW>* s = t.slots + idx;
     U128 cur = claimed ? U128{PAYLOAD_FRESH, EMPTY64} : ldcg128(&s->payload);
-    slot_apply(s, cur.a, cur.b, left, right, rank);
+    slot_apply(s, cur.a, cur.b, left, right, rank, c);
     return claimed;
 }
 // K <= 63: the whole 32 B slot arrives with one sector read per probe (ld256), so a hit needs no second read before the CAS and
 // a fresh claim knows the {payload, rank} it will find (the memset state).
 template <>
-PG_D bool table_insert<2>(const Table<2>& t, const Kmer<2>& k, unsigned left, unsigned right, u64 rank, u64* idx_out) {
+PG_D bool table_insert<2>(const Table<2>& t, const Kmer<2>& k, unsigned left, unsigned right, u64 rank, u64* idx_out, unsigned c) {
     u64 idx = table_hash(k) & t.mask;
     bool claimed = false;
     U128 cur;
@@ -280,7 +303,7 @@ PG_D bool table_insert<2>(const Table<2>& t, const Kmer<2>& k, unsigned left, un
         idx = (idx + 1) & t.mask;
     }
     if (idx_out) *idx_out = idx;
-    slot_apply(s, cur.a, cur.b, left, right, rank);
+    slot_apply(s, cur.a, cur.b, left, right, rank, c);
     return claimed;
 }
 
