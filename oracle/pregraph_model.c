@@ -11,9 +11,10 @@
  * The reference ships no tests / golden vectors of its own (SURVEY.md section 4), so that binary is the pin.
  *
  * Build:  gcc -O2 -DMODEL_W=128 (63-mer build, Kmer = 2 x u64)   |  -DMODEL_W=256 (127-mer build, 4 x u64)
- * Usage:  pregraph_model_63 -s cfg -o prefix [-K k] [-p P] [-a G] [-d D] [-R] [-T table_dump.bin] [-1]
+ * Usage:  pregraph_model_63 -s cfg -o prefix [-K k] [-p P] [-a G] [-d D] [-R] [-T table_dump.bin] [-U tips_dump.bin] [-1]
  *         -T : dump {kmer words, l[4], r[4], cov, flags} of every node in reference iteration order
  *              right after pass 1 + mark-linear (before tips) -- the intermediate the CUDA kernels are checked on.
+ *         -U : the same records right after tip removal (before the edges clear links and overlay edge ids).
  *         -1 : stop after pass 1 (.kmerFreq only); used by the cpu_baseline timing leg.
  *
  * Supported input domain (same as the engine's): single-line FASTA, 4-line FASTQ, files ending in '\n',
@@ -585,13 +586,13 @@ static void self_kats(void) {
 }
 
 int main(int argc, char **argv) {
-    const char *cfg = NULL, *tdump = NULL; int only1 = 0, c; K = 23;
+    const char *cfg = NULL, *tdump = NULL, *udump = NULL; int only1 = 0, c; K = 23;
     if (argc > 1 && !strcmp(argv[1], "-V")) { self_kats(); return 0; }
     if (argc > 1 && !strcmp(argv[1], "pregraph")) { argv++; argc--; }
-    while ((c = getopt(argc, argv, "a:s:o:K:p:d:RT:1")) != -1) switch (c) {
+    while ((c = getopt(argc, argv, "a:s:o:K:p:d:RT:U:1")) != -1) switch (c) {
         case 's': cfg = optarg; break; case 'o': prefix = optarg; break; case 'K': K = atoi(optarg); break;
         case 'p': P = atoi(optarg); break; case 'R': repsTie = 1; break; case 'd': D = atoi(optarg) >= 0 ? atoi(optarg) : 0; break;
-        case 'a': initG = atoi(optarg); break; case 'T': tdump = optarg; break; case '1': only1 = 1; break;
+        case 'a': initG = atoi(optarg); break; case 'T': tdump = optarg; break; case 'U': udump = optarg; break; case '1': only1 = 1; break;
     }
     if (!cfg || !prefix) { fprintf(stderr, "usage: pregraph_model -s cfg -o prefix [-K k -p P -a G -d D -R]\n"); return -1; }
     /* pregraph.c:71-97 */
@@ -610,6 +611,8 @@ int main(int argc, char **argv) {
     fprintf(stderr, "model: pass1 %.3fs\n", (t0.tv_sec - t1.tv_sec) + 1e-9 * (t0.tv_nsec - t1.tv_nsec));
     if (tdump) dump_table(tdump);
     if (only1) return 0;
-    tips(); edges(); pass2(); vertices();
+    tips();
+    if (udump) dump_table(udump);
+    edges(); pass2(); vertices();
     return 0;
 }

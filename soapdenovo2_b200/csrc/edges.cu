@@ -195,6 +195,10 @@ struct EmIn {
     const EdgeRec* rec;
     __device__ u64 operator()(u64 j) const { return rec[j].status == 1; }
 };
+struct EmNoRevIn {   // emitted starts whose far end is a deleted node (nothing to claim)
+    const EdgeRec* rec;
+    __device__ u64 operator()(u64 j) const { return rec[j].status == 1 && rec[j].rev_id == EMPTY64; }
+};
 struct PrefixOut {
     u64* out;
     __device__ void operator()(u64 j, u64 prefix, u64) const { out[j] = prefix; }
@@ -295,7 +299,9 @@ void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
     // who emits: rounds of claim / resolve
     claimb.alloc((S + 1) * sizeof(u64));
     u64* claim = claimb.template as<u64>();
+    int rounds = 0;
     for (int round = 0;; round++) {
+        rounds = round + 1;
         PG_CUDA(cudaMemsetAsync(claim, 0xFF, (S + 1) * sizeof(u64), st_));
         PG_CUDA(cudaMemsetAsync(err + 1, 0, sizeof(u64), st_));
         k_edge_claim<<<blocks, 256, 0, st_>>>(starts, S, rec, claim);
@@ -345,6 +351,12 @@ void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
         device_scan(EmIn{rec}, NullOut{}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
         read_counters();
         st->edges = h_cnt_[C_MISC0];
+    }
+    if (prm_.verbose) {
+        device_scan(EmNoRevIn{rec}, NullOut{}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
+        read_counters();
+        fprintf(stderr, "[pgb200] build_edges: %llu start(s), %d claim/resolve round(s), %llu emitted start(s) without a reverse start\n",
+                (unsigned long long)S, rounds, (unsigned long long)h_cnt_[C_MISC0]);
     }
 }
 

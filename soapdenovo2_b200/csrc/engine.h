@@ -48,6 +48,14 @@ struct TipStats {
     std::vector<uint64_t> minor_cycles;
     uint64_t minor_tips = 0, minor_relinear = 0;
     uint64_t rounds = 0;
+    // how the parallel restatement got there (printed under PGB200_VERBOSE; tests use them to show a branch ran)
+    uint64_t thin_rounds = 0;         // k_thin_commit rounds
+    uint64_t minor_windows = 0;       // speculated windows over all minor sweeps
+    uint64_t dirty_frontiers = 0;     // windows cut short by a candidate that read a node a smaller pending clip writes
+    uint64_t barrier_frontiers = 0;   // windows cut short by a node a committed clip turned into a dead end further down the sweep
+    uint64_t requeued = 0;            // candidates put back into the pending "extra" set (window survivors and new dead ends)
+    uint64_t deadends_ahead = 0;      // new dead ends queued for the sweep that made them
+    uint64_t deadends_behind = 0;     // new dead ends behind the clip that made them: the next sweep visits them (counted under verbose)
 };
 
 struct EdgeStats {

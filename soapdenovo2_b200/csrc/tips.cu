@@ -345,6 +345,7 @@ void EngineT<NW>::remove_tips(TipStats* st) {
                 PG_CUDA(cudaGetLastError());
                 read_counters();
                 st->rounds++;
+                st->thin_rounds++;
                 if (h_cnt_[C_MISC1] == 0) break;
                 if (round > 64) throw std::runtime_error("pgb200: THIN tip resolution did not converge");
             }
@@ -358,6 +359,9 @@ void EngineT<NW>::remove_tips(TipStats* st) {
     u64* ctl = ctlb.template as<u64>();
     DevBuf winb, win2b;
     u64 total_minor = 0;
+    // PGB200_TIP_WINDOW=n: every window takes n list entries (no adaptation).  The result is the same at any n; n = 1..3 cut every
+    // conflict across windows, so that tests reach the dirty / barrier / re-queue paths on small graphs.
+    const u64 fixed_window = getenv("PGB200_TIP_WINDOW") ? (u64)std::max(1L, atol(getenv("PGB200_TIP_WINDOW"))) : 0;
     for (int sweep = 0;; sweep++) {
         u64 nc = build_cands(false);
         u64 clipped = 0;
@@ -365,7 +369,7 @@ void EngineT<NW>::remove_tips(TipStats* st) {
             // pending candidates: a static sorted list (cand[lo..nc)) plus a small unsorted "extra" set
             std::vector<u64> h_extra;
             u64 lo = 0;
-            u64 Wn = 4096;
+            u64 Wn = fixed_window ? fixed_window : 4096;
             std::vector<u64> h_cand;   // fetched lazily in pieces
             while (lo < nc || !h_extra.empty()) {
                 // window = next Wn list entries + every extra below the window end
@@ -399,6 +403,12 @@ void EngineT<NW>::remove_tips(TipStats* st) {
                 sync();
                 clipped += h_ctl[2];
                 st->rounds++;
+                st->minor_windows++;
+                if (frontier < wend) {
+                    if (frontier == h_ctl[0]) st->dirty_frontiers++;
+                    else st->barrier_frontiers++;
+                }
+                const u64 survivors_extra = (u64)std::count_if(ex_in.begin(), ex_in.end(), [&](u64 e) { return e >= frontier; });
                 // survivors of the window (ord >= frontier) + new dead ends
                 std::vector<u64> back(h_ctl[3]);
                 if (h_ctl[3]) PG_CUDA(cudaMemcpyAsync(back.data(), win2b.p, h_ctl[3] * sizeof(u64), cudaMemcpyDeviceToHost, st_));
@@ -417,11 +427,23 @@ void EngineT<NW>::remove_tips(TipStats* st) {
                     back.swap(keep);
                 }
                 lo += committed_list;
+                st->requeued += back.size();
+                st->deadends_ahead += back.size() - survivors_extra;
+                if (prm_.verbose) {   // committed clips that made a new dead end, ahead or behind (rec and win are still those of this window)
+                    std::vector<TipRec> hr(nwin);
+                    std::vector<u64> hw(nwin);
+                    PG_CUDA(cudaMemcpyAsync(hr.data(), rec, nwin * sizeof(TipRec), cudaMemcpyDeviceToHost, st_));
+                    PG_CUDA(cudaMemcpyAsync(hw.data(), win, nwin * sizeof(u64), cudaMemcpyDeviceToHost, st_));
+                    sync();
+                    u64 made = 0;
+                    for (u64 i = 0; i < nwin; i++) made += hw[i] < frontier && hr[i].state == 1 && (hr[i].code & 16u);
+                    st->deadends_behind += made - (back.size() - survivors_extra);
+                }
                 h_extra = ex_out;
                 for (u64 e : back) h_extra.push_back(e);
                 // adapt the window to the observed commit run length
                 u64 done = committed_list;
-                Wn = std::min<u64>(1u << 18, std::max<u64>(1024, done * 2));
+                if (!fixed_window) Wn = std::min<u64>(1u << 18, std::max<u64>(1024, done * 2));
                 if (st->rounds > (1ull << 26)) throw std::runtime_error("pgb200: minor tip sweeps did not converge");
             }
         }
@@ -432,6 +454,11 @@ void EngineT<NW>::remove_tips(TipStats* st) {
     }
     st->minor_tips = total_minor;
     st->minor_relinear = remark();
+    if (prm_.verbose)
+        fprintf(stderr, "[pgb200] remove_tips: %llu THIN round(s), %llu minor window(s), %llu dirty frontier(s), %llu barrier frontier(s), "
+                "%llu re-queued, %llu new dead end(s) queued ahead, %llu behind\n", (unsigned long long)st->thin_rounds,
+                (unsigned long long)st->minor_windows, (unsigned long long)st->dirty_frontiers, (unsigned long long)st->barrier_frontiers,
+                (unsigned long long)st->requeued, (unsigned long long)st->deadends_ahead, (unsigned long long)st->deadends_behind);
 }
 
 template void EngineT<2>::remove_tips(TipStats*);

@@ -363,3 +363,297 @@ def config_c5(d: str, genome_len=20_000_000, seed=5) -> str:
         {"avg_ins": 2000, "reverse_seq": 1, "asm_flags": 3, "files": [("f", j("c5_c.fa")), ("q", j("c5_d.fq"))]},
     ])
     return cfg
+
+
+# ---------------------------------------------------------------- graph motifs for the tip and edge phases
+# Error-free reads on fresh random sequence, so that every link's multiplicity is exactly the number of reads that cross it.
+# A "ring" is a circular backbone covered by reads of length K + c*s tiled every s bases: every ring link is crossed by exactly c
+# reads and the ring has no dead end.  Branches hang off ring k-mers ("junctions"); each branch string is read `copies` times whole.
+MOTIFS = ("cut", "tie", "conflict", "cascade", "isolated", "thin_orphan", "thin_multi", "lollipop", "hairpin", "figure8", "bubble",
+          "ring", "large", "barrier")
+_TILE = 10
+
+
+class _Motifs:
+    def __init__(self, K: int, seed: int):
+        self.K, self.rng = K, np.random.default_rng(seed)
+        self.reads: list[tuple[bytes, int]] = []       # (sequence, copies)
+        self.walks: list[tuple[bytes, int, bytes]] = []  # claimed tip walks: (dead-end k-mer, linear nodes walked, k-mer it stops at)
+        self.expect = {"nodes": 0, "dead_ends": 0, "junctions": 0}
+
+    def seq(self, n: int) -> bytes:
+        return _ACGT[self.rng.integers(0, 4, size=n)].tobytes()
+
+    def other(self, *avoid) -> bytes:
+        return bytes([int(self.rng.choice([b for b in b"ACGT" if b not in avoid]))])
+
+    def ring(self, G: int, c: int) -> bytes:
+        G = -(-max(G, self.K + 2) // _TILE) * _TILE
+        C = self.seq(G)
+        R = self.K + c * _TILE
+        C2 = C * (R // G + 2)
+        for j in range(0, G, _TILE):
+            self.reads.append((C2[j:j + R], 1))
+        self.expect["nodes"] += G
+        return C
+
+    def kmer(self, C: bytes, p: int) -> bytes:
+        return (C * (self.K // len(C) + 2))[p % len(C):p % len(C) + self.K]
+
+    def left_tip(self, C: bytes, p: int, m: int, copies: int, avoid=b"") -> bytes:
+        """a branch of m linear nodes and a dead end arriving at ring k-mer p from its left"""
+        J = self.kmer(C, p)
+        T = self.seq(m) + self.other(C[(p - 1) % len(C)], *avoid)
+        self.reads.append((T + J, copies))
+        self.walks.append(((T + J)[:self.K], m, J))
+        self.expect["nodes"] += m + 1
+        self.expect["dead_ends"] += 1
+        return T
+
+    def right_tip(self, C: bytes, p: int, m: int, copies: int, avoid=b"") -> bytes:
+        J = self.kmer(C, p)
+        T = self.other(C[(p + self.K) % len(C)], *avoid) + self.seq(m)
+        self.reads.append((J + T, copies))
+        self.walks.append((_rc_bytes((J + T)[-self.K:]), m, _rc_bytes(J)))
+        self.expect["nodes"] += m + 1
+        self.expect["dead_ends"] += 1
+        return T
+
+    def tip(self, C, p, m, copies):
+        return (self.left_tip if self.rng.random() < 0.5 else self.right_tip)(C, p, m, copies)
+
+
+def _rc_bytes(s: bytes) -> bytes:
+    return _COMP[np.frombuffer(s, dtype=np.uint8)[::-1]].tobytes()
+
+
+def _motif(M: _Motifs, kind: str, i: int) -> None:
+    """one instance of `kind` (i: instance number, picks the variant)"""
+    K, e = M.K, M.expect
+    if kind == "cut":            # chains of 2K-2 .. 2K+1 linear nodes: clipped up to 2K-1
+        C = M.ring(2 * K, 3)
+        M.tip(C, 0, 2 * K - 2 + i % 4, 2)
+        e["junctions"] += 1
+    elif kind == "tie":          # the tip's link equals the ring's (kept) or is one below (clipped)
+        C = M.ring(2 * K, 3)
+        M.tip(C, 0, K, 3 if i % 2 == 0 else 2)
+        e["junctions"] += 1
+    elif kind == "conflict":     # 2 or 3 tips into J1; J1 -> path -> J2 on a ring; after the first clip(s) J1 is linear
+        ntips = 2 + i % 2
+        covs = [2, 3, 4][:ntips]
+        near = (i // 2) % 2 == 0        # the last tip's walk reaches J2 (else it passes 2K nodes and gives up)
+        cr = sum(covs) + (i // 4) % 2   # J2: the merged branch ties with the ring or is one below it
+        C = M.ring(2 * K, cr)
+        J2 = M.kmer(C, 0)
+        d = 1 if near else 2 * K
+        J1 = M.seq(K)
+        P = M.seq(d - 1) + M.other(C[-1]) if d > 1 else M.other(C[-1], J1[-1:][0])
+        used = b""
+        for c in covs:
+            m = int(M.rng.integers(1, max(2, K - 2 - d)))
+            T = M.seq(m) + M.other(*used)
+            used += T[-1:]
+            M.reads.append((T + J1 + P + J2, c))
+            M.walks.append(((T + J1 + P + J2)[:K], m, J1))
+            e["nodes"] += m + 1
+        e["nodes"] += K + d              # J1 and the d + K - 1 linear nodes on to J2
+        e["dead_ends"] += ntips
+        e["junctions"] += 2
+    elif kind == "cascade":      # A3 -> J3 <- Q3 - J2 - Q2 -> J1 <- Q1 - J0 (ring): each clip turns the next junction into a dead end
+        C = M.ring(2 * K, 6)
+        J0 = M.kmer(C, 0)
+        J1, J2, J3 = M.seq(K), M.seq(K), M.seq(K)
+        u = lambda: int(M.rng.integers(1, K // 2 + 1))
+        U1 = M.other(C[K % len(C)]) + M.seq(u())
+        U2 = M.seq(u())
+        U3 = M.other(U2[0]) + M.seq(u())
+        U2 = U2[:-1] + M.other(U1[-1]) if len(U2) > 1 else M.other(U1[-1], U3[0])
+        M.reads += [(J0 + U1 + J1, 5), (J2 + U2 + J1, 4), (J2 + U3 + J3, 3)]
+        m = int(M.rng.integers(1, 2 * K))
+        T = M.seq(m) + M.other(U3[-1])
+        M.reads.append((T + J3, 2))
+        M.walks.append(((T + J3)[:K], m, J3))
+        e["nodes"] += 3 * K + len(U1) + len(U2) + len(U3) - 3 + 3 + m + 1
+        e["dead_ends"] += 1
+        e["junctions"] += 4
+    elif kind == "isolated":     # a lone path: both ends are dead ends; 2K-2 .. 2K+1 linear nodes between them
+        m = 2 * K - 2 + i % 4
+        S = M.seq(m + K + 1)
+        M.reads.append((S, 2))
+        M.walks.append((S[:K], m, _rc_bytes(S[-K:])))
+        e["nodes"] += m + 2
+        e["dead_ends"] += 2
+    elif kind == "thin_orphan":  # a frequency-one tip whose last h nodes a second read covers: THIN stops at a non-single node
+        C = M.ring(2 * K, 3)
+        m = int(M.rng.integers(K // 2 + 2, 2 * K - 1))
+        T = M.left_tip(C, 0, m, 1)
+        h = int(M.rng.integers(1, min(m, K)))
+        M.reads.append(((T + M.kmer(C, 0))[-(K + h):], 1))
+        e["junctions"] += 1
+    elif kind == "thin_multi":   # three frequency-one tips on each side of one ring k-mer: one THIN commit per round and junction
+        C = M.ring(2 * K, 3)
+        l, r = b"", b""
+        for _ in range(3):
+            l += M.left_tip(C, 0, int(M.rng.integers(1, 2 * K)), 1, avoid=l)[-1:]
+            r += M.right_tip(C, 0, int(M.rng.integers(1, 2 * K)), 1, avoid=r)[:1]
+        e["junctions"] += 1
+    elif kind == "lollipop":     # a loop leaving and re-entering one junction, with a tail too long to clip
+        C = M.ring(2 * K, 3)
+        M.tip(C, 0, 2 * K + 3, 2)
+        e["junctions"] += 1
+    elif kind == "hairpin":      # J -> w -> rc(w) -> rc(J): a unipath that folds back onto itself and re-enters J by the same link
+        C = M.ring(2 * K, 3)
+        J = M.kmer(C, 0)
+        w = M.other(C[K % len(C)]) + M.seq(int(M.rng.integers(1, 2 * K)))
+        M.reads.append((J + w + _rc_bytes(J + w), 2))
+        e["nodes"] += len(w) + (K - 1) // 2   # J + w + rc(J + w) has len(w) + (K + 1) / 2 distinct k-mers, J among them
+        e["junctions"] += 1
+    elif kind == "figure8":      # two rings through one k-mer
+        J = M.seq(K)
+        G = -(-2 * K // _TILE) * _TILE
+        a = M.seq(G - K)
+        b = M.other(a[0]) + M.seq(len(a) - 2) + M.other(a[-1])
+        for x in (a, b):
+            C = J + x
+            R = K + 3 * _TILE
+            C2 = C * (R // G + 2)
+            M.reads += [(C2[j:j + R], 1) for j in range(0, G, _TILE)]
+        e["nodes"] += 2 * G - 1
+        e["junctions"] += 1
+    elif kind == "bubble":       # J1 -> J2 along the ring (d steps) and along a bypass (t+K steps); d = 1 is a length-1 edge
+        lens = [x for x in (100, 101, 200, 201) if x > K]
+        d = [1, 100, 101, 200][i % 4]
+        L = lens[(i // 4) % len(lens)]
+        C = M.ring(d + 2 * K + 20, 3)
+        J1, J2 = M.kmer(C, 0), M.kmer(C, d)
+        t = L - K
+        v = M.other(C[K]) + M.seq(t - 2) + M.other(C[d - 1]) if t >= 2 else M.other(C[K], C[d - 1])
+        M.reads.append((J1 + v + J2, 3))
+        e["nodes"] += t + K - 1
+        e["junctions"] += 2
+    elif kind == "barrier":      # A's clip turns X into a dead end; X's clip at Y makes Y linear; tip c, a tie at Y before, then
+        C = M.ring(2 * K, 8)     # walks on to Z and is clipped there: in the same sweep only if c comes after X in iteration order
+        Z = M.kmer(C, 0)
+        Y, X = M.seq(K), M.seq(K)
+        P = M.other(C[K % len(C)])
+        Q = M.seq(int(M.rng.integers(1, K + 1)))
+        mc = int(M.rng.integers(1, K - 2))
+        Tc = M.other(Q[0]) + M.seq(mc)
+        M.reads += [(Z + P + Y + Q + X, 3), (Z + P + Y + Tc, 4)]
+        M.walks.append((_rc_bytes((Y + Tc)[-K:]), mc, _rc_bytes(Y)))
+        mA = int(M.rng.integers(1, 2 * K))
+        T = M.seq(mA) + M.other(Q[-1])
+        M.reads.append((T + X, 2))
+        M.walks.append(((T + X)[:K], mA, X))
+        e["nodes"] += (K + 1) + (len(Q) + K) + (mc + 1) + (mA + 1)
+        e["dead_ends"] += 2
+        e["junctions"] += 3
+    elif kind == "ring":         # no branch at all: no edge, no vertex
+        M.ring(2 * K, 3)
+    elif kind == "large":        # a long ring with a short minority tip every 12 bases: thousands of minor candidates per ring
+        n = 40
+        C = M.ring(n * 12, 3)
+        for j in range(n):
+            M.tip(C, 12 * j, 3, 2)
+        e["junctions"] += n
+    else:
+        raise ValueError(kind)
+
+
+def motif_reads(kind: str, K: int, copies: int, seed: int = 0) -> _Motifs:
+    """`copies` instances of one motif on fresh random sequence; .reads, .walks and .expect describe what was built"""
+    M = _Motifs(K, seed * 1000 + MOTIFS.index(kind) * 7 + K)
+    for i in range(copies):
+        _motif(M, kind, i)
+    return M
+
+
+def write_motif_scenario(d: str, kinds, K: int, copies: int, seed: int = 0) -> tuple[str, list]:
+    """One FASTA library holding `copies` instances of each motif in `kinds` (reads shuffled); returns (config path, motif sets).
+    The reads are checked first (check_motifs): a chance k-mer collision between instances would make a different graph."""
+    sets = [motif_reads(k, K, copies, seed) for k in kinds]
+    check_motifs(sets, K)
+    rng = np.random.default_rng(seed + 17 * K)
+    reads = [s for M in sets for s, c in M.reads for _ in range(c)]
+    order = rng.permutation(len(reads))
+    fa = os.path.join(d, "motif.fa")
+    with open(fa, "wb") as f:
+        for n, j in enumerate(order):
+            f.write(b">m%d\n" % n + reads[j] + b"\n")
+    _pad_if_32k(fa)
+    cfg = os.path.join(d, "motif.cfg")
+    write_config(cfg, max(len(r) for r in reads), [{"avg_ins": 200, "files": [("f", fa)]}])
+    return cfg, sets
+
+
+_CODE = {65: 0, 67: 1, 84: 2, 71: 3}             # the reference's 2-bit codes: A0 C1 T2 G3 (complement = code ^ 2)
+_ORD = bytes.maketrans(b"ACTG", b"abcd")          # byte order == code order, so canonical = the smaller translated string
+
+
+def _canon(k: bytes) -> tuple[bytes, bool]:
+    r = _rc_bytes(k)
+    return (k, True) if k.translate(_ORD) < r.translate(_ORD) else (r, False)
+
+
+def debruijn(reads, K: int) -> dict:
+    """The canonical k-mer graph of (sequence, copies) reads as pass 1 builds it: node -> [l[4], r[4]], counters capped at 63."""
+    g: dict = {}
+    for s, copies in reads:
+        for j in range(len(s) - K + 1):
+            k, fwd = _canon(s[j:j + K])
+            prev = _CODE[s[j - 1]] if j > 0 else None
+            nxt = _CODE[s[j + K]] if j + K < len(s) else None
+            if not fwd:
+                prev, nxt = (nxt ^ 2 if nxt is not None else None), (prev ^ 2 if prev is not None else None)
+            lr = g.setdefault(k, [[0] * 4, [0] * 4])
+            if prev is not None:
+                lr[0][prev] = min(63, lr[0][prev] + copies)
+            if nxt is not None:
+                lr[1][nxt] = min(63, lr[1][nxt] + copies)
+    return g
+
+
+def _degree(lr):
+    return sum(1 for x in lr[0] if x), sum(1 for x in lr[1] if x)
+
+
+def graph_shape(g: dict) -> dict:
+    shape = {"nodes": len(g), "dead_ends": 0, "junctions": 0}
+    for lr in g.values():
+        i, o = _degree(lr)
+        if i + o == 1:
+            shape["dead_ends"] += 1
+        elif not (i == 1 and o == 1):
+            shape["junctions"] += 1
+    return shape
+
+
+def tip_walk(g: dict, start: bytes, K: int) -> tuple[int, bytes]:
+    """From a dead end over linear nodes: (linear nodes passed, canonical k-mer of the first non-linear node)"""
+    cur, _ = _canon(start)
+    i, o = _degree(g[cur])
+    assert i + o == 1, f"{start!r} is not a dead end"
+    ori = cur if o == 1 else _rc_bytes(cur)        # oriented so that its one link points right
+    m = 0
+    while True:
+        k, fwd = _canon(ori)
+        lr = g[k]
+        if m or k != cur:
+            i, o = _degree(lr)
+            if not (i == 1 and o == 1):
+                return m, k
+            m += 1
+        c = next(c for c in range(4) if lr[1][c]) if fwd else next(c for c in range(4) if lr[0][c]) ^ 2
+        ori = ori[1:] + b"ACTG"[c:c + 1]
+
+
+def check_motifs(sets, K: int) -> dict:
+    """Asserts that the reads of the motif sets build the graph they claim: node, dead-end and junction counts, and every claimed
+    tip walk's length and end node.  Returns the graph."""
+    g = debruijn([r for M in sets for r in M.reads], K)
+    want = {k: sum(M.expect[k] for M in sets) for k in ("nodes", "dead_ends", "junctions")}
+    assert graph_shape(g) == want, (graph_shape(g), want)
+    for M in sets:
+        for start, m, end in M.walks:
+            assert tip_walk(g, start, K) == (m, _canon(end)[0]), (start, m, end)
+    return g
