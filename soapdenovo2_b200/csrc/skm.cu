@@ -25,11 +25,11 @@ namespace pgb {
 
 constexpr int SKM_PART_THREADS = 128;
 constexpr int SKM_APPLY_THREADS = 256;
-// Shared-memory table of a bucket: 1024 slots (32 KB at K <= 63) plus the record stage (2 x SKM_STAGE_RECS = 64 records), the
-// distinct-record buffer (SKM_BUF_RECS = 128 records, their reversed bases, counts and dedup table) put 4 CTAs = 32 warps on an H100
-// SM (4 x 48 KB of 228 KB) at 64 registers per thread; 256-bit keys (48 B slots, 71 KB per CTA) run 3 CTAs at 72 registers.  No stack
-// frame and no spills at either width.  The stage was 2 x 128 records before the buffer existed; halving it pays for the buffer at
-// K > 63.  5 or 6 CTAs spill at the register budget they allow.
+// Shared-memory table of a bucket: 1024 slots (32 KB at K <= 63) plus the record stage (2 x 128 records), the distinct-record buffer
+// (SKM_BUF_RECS = 128 records, their reversed bases, counts and a 512-slot dedup table) put 4 CTAs = 32 warps on an H100 SM
+// (4 x 54 KB of 228 KB) at 64 registers per thread; 256-bit keys (48 B slots, a 2 x 64-record stage, a 256-slot dedup table, 71 KB
+// per CTA) run 3 CTAs at 74.  No stack frame and no spills at either width (skm_w).  5 or 6 CTAs spill at the register budget they
+// allow.
 #ifndef SKM_LOG2_SLOTS
 #define SKM_LOG2_SLOTS 10
 #endif
@@ -378,20 +378,42 @@ struct SkmApplyArgs {
     u64* hist;                // [256] coverage histogram of the swept entries
     u64* spill_list;          // slots of the keys stored unswept (spilled instances): the host sweeps them afterwards
     u64 spill_cap;
+    int collapse;             // SKM_COLLAPSE_OFF / _ON / _AUTO (PGB200_SKM_COLLAPSE): both ways of filling the buffer are exact.  256-bit
+                              // keys only: at K <= 63 records repeat (0.553 of them distinct at 30x) and the kernel always collapses;
+                              // its register budget at 4 CTAs per SM has no room for the copy path (DESIGN.md §5)
 };
 constexpr u64 SKM_CREDIT = 1ull << 16;   // table room a CTA reserves at a time (keys)
+constexpr int SKM_COLLAPSE_OFF = 0, SKM_COLLAPSE_ON = 1, SKM_COLLAPSE_AUTO = 2;
+// auto: a CTA measures its distinct / staged records over SKM_AUTO_PROBE collapsed buckets; above SKM_AUTO_NUM / SKM_AUTO_DEN the
+// records hardly repeat and it copies the next SKM_AUTO_SKIP buckets' records straight into the buffer, then measures again
+constexpr u32 SKM_AUTO_PROBE = 8, SKM_AUTO_SKIP = 56, SKM_AUTO_NUM = 9, SKM_AUTO_DEN = 10;
 
 // -DSKM_PHASE_CLOCKS: k_skm_apply adds up clock64() per phase over all its threads (stage wait, instance build, find / claim, apply,
-// spill to the global table, flush, record dedup); the host prints the totals of every aggregation with PGB200_SKM_STATS.  Off: no
-// code at all.
+// spill to the global table, flush, record dedup), and thread 0 of every CTA splits the CTA's wall time between two of its
+// barrier-delimited boundaries into SKM_WALL_PHASES phases that cover the whole kernel; the host prints both splits of every
+// aggregation with PGB200_SKM_STATS.  Off: no code at all.
 #ifdef SKM_PHASE_CLOCKS
 constexpr int SKM_PHASES = 7;
 __device__ unsigned long long g_skm_phase_clk[SKM_PHASES];
 #define SKM_T0(v) const long long v = clock64()
 #define SKM_ACC(i, v) clk[i] += (u64)(clock64() - (v))
+// wall phases: top of bucket (scan + credit), stage wait, dedup or copy of a window incl. its barrier, drain pre-pass, drain steps
+// incl. the barrier, flush incl. the barrier, other; then the kernel's end minus start and the number of CTAs (the check: the
+// phases sum to it)
+constexpr int SKM_WALL_PHASES = 7;
+__device__ unsigned long long g_skm_wall_clk[SKM_WALL_PHASES + 2];
+#define SKM_WALL(i)                                      \
+    do {                                                 \
+        if (tid == 0) {                                  \
+            const long long t_ = clock64();              \
+            s_wall[i] += (u64)(t_ - s_wall_last);        \
+            s_wall_last = t_;                            \
+        }                                                \
+    } while (0)
 #else
 #define SKM_T0(v)
 #define SKM_ACC(i, v)
+#define SKM_WALL(i)
 #endif
 
 // Exclusive prefix sum over the CTA; *total = the sum.  The caller separates two calls with a __syncthreads (s_warp is reused).
@@ -420,14 +442,27 @@ __device__ __forceinline__ u32 cta_exclusive_scan(u32 v, u32* s_warp, u32& total
 // segment thread copies its part of the window with one bulk copy, completed on the half's mbarrier.  The stage is double-buffered:
 // the next window (or the next bucket's first) is in flight while the current one is processed and synchronised.  A window is only
 // collapsed into the distinct-record buffer (skm_dedup_insert), so the stage just has to keep the bulk copies ahead.
-#ifndef SKM_STAGE_RECS
-#define SKM_STAGE_RECS 64
+// Records per window: 128 at K <= 63 (2 x 4 KB of stage; a bucket's ~210 records at 30x take 2 windows instead of 4, so half the
+// window barriers, and 128 threads collapse a window instead of 64), 64 at K > 63 (2 x 3 KB: what 3 CTAs per SM leave).
+#ifndef SKM_STAGE_RECS_NW2
+#define SKM_STAGE_RECS_NW2 128
 #endif
-constexpr int SKM_W = SKM_STAGE_RECS;
+#ifndef SKM_STAGE_RECS_NW4
+#define SKM_STAGE_RECS_NW4 64
+#endif
 constexpr int SKM_BUF_RECS = 128;        // distinct records buffered before they are expanded into k-mer instances (a drain)
-constexpr int SKM_DEDUP_SLOTS = 256;     // the buffer's hash table: record -> buffer position
-static_assert(SKM_W <= SKM_BUF_RECS && SKM_BUF_RECS <= SKM_APPLY_THREADS, "one drain empties the buffer for a whole window; one thread per buffered record");
-static_assert(SKM_BUF_RECS + SKM_W < SKM_DEDUP_SLOTS && (SKM_DEDUP_SLOTS & (SKM_DEDUP_SLOTS - 1)) == 0, "the dedup table never fills up");
+template <int NW>
+__host__ __device__ constexpr int skm_w() { return NW == 2 ? SKM_STAGE_RECS_NW2 : SKM_STAGE_RECS_NW4; }
+// the buffer's hash table (record -> buffer position): room for the buffered records and the FULL marks of one window, never full
+template <int NW>
+__host__ __device__ constexpr int skm_dd_slots() { return SKM_BUF_RECS + skm_w<NW>() < 256 ? 256 : 512; }
+template <int NW>
+__host__ __device__ constexpr bool skm_stage_ok() {
+    return skm_w<NW>() <= SKM_BUF_RECS && SKM_BUF_RECS <= SKM_APPLY_THREADS && SKM_BUF_RECS % skm_w<NW>() == 0 &&
+           SKM_BUF_RECS + skm_w<NW>() < skm_dd_slots<NW>();
+}
+static_assert(skm_stage_ok<2>() && skm_stage_ok<4>(), "one drain empties the buffer for a whole window, one thread per buffered record, "
+                                                      "uncollapsed windows fill the buffer exactly, the dedup table never fills up");
 
 constexpr u32 SKM_DD_EMPTY = 0xFFFFFFFFu, SKM_DD_BUSY = 0xFFFFFFFEu, SKM_DD_FULL = 0xFFFFFFFDu;
 // One staged record r into the distinct-record buffer: find-or-claim its entry in the dedup table (claim: CAS EMPTY -> BUSY, take
@@ -438,7 +473,8 @@ template <int NW>
 __device__ __forceinline__ bool skm_dedup_insert(const u64* r, u64* buf, u32* cnt, u32* dd, u32* nbuf) {
     constexpr int RW = NW + 2;
     volatile u32* vdd = dd;
-    u32 idx = skm_rec_hash<NW>(r) >> (32 - __builtin_ctz(SKM_DEDUP_SLOTS));
+    constexpr int DS = skm_dd_slots<NW>();
+    u32 idx = skm_rec_hash<NW>(r) >> (32 - __builtin_ctz(DS));
     for (;;) {
         u32 v = vdd[idx];
         if (v == SKM_DD_EMPTY) {
@@ -468,7 +504,7 @@ __device__ __forceinline__ bool skm_dedup_insert(const u64* r, u64* buf, u32* cn
             atomicMin((unsigned long long*)&buf[v * RW], (unsigned long long)r[0]);
             return false;
         }
-        idx = (idx + 1) & (SKM_DEDUP_SLOTS - 1);
+        idx = (idx + 1) & (DS - 1);
     }
 }
 
@@ -478,7 +514,7 @@ struct SkmSegRange {
 };
 // Queue window w of a bucket of R records into a stage half.  Every thread calls it: thread 0 arrives with the window's byte count,
 // the segment threads whose range meets the window copy their part.
-template <int RW>
+template <int RW, int SKM_W>
 __device__ __forceinline__ void skm_stage_window(u64* stage, u64* bar, const u64* my_recs, const SkmSegRange& sr, u32 R, u32 w) {
     const u32 a = w * (u32)SKM_W, e = min(R, a + (u32)SKM_W);
     if (threadIdx.x == 0) mbar_expect_tx(bar, (e - a) * (u32)(RW * sizeof(u64)));
@@ -501,7 +537,8 @@ __device__ __forceinline__ void skm_stage_window(u64* stage, u64* bar, const u64
 // two shifts of shared-memory words (skm_instance_staged) and applies it as many times as its record occurred.
 template <int NW>
 __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k_skm_apply(Table<NW> tab, KParams<NW> kp, SkmApplyArgs a) {
-    constexpr int RW = NW + 2, WARPS = SKM_APPLY_THREADS / 32, C = SKM_BUF_RECS;
+    constexpr int RW = NW + 2, WARPS = SKM_APPLY_THREADS / 32, C = SKM_BUF_RECS, SKM_W = skm_w<NW>(), SKM_DEDUP_SLOTS = skm_dd_slots<NW>();
+    constexpr bool COPY_PATH = NW > 2;   // SKM_COLLAPSE_OFF / _AUTO exist for 256-bit keys only (see SkmApplyArgs::collapse)
     // key[NW][S], pay[S], rnk[S], stage[2][W][RW], buf[C][RW], rv[C][NW+1], list[S] (u16), P[C+1], cnt[C], dedup[DS]
     extern __shared__ __align__(16) u64 s_dyn[];
     u64* const s_stage = s_dyn + (NW + 2) * SKM_SLOTS;
@@ -517,7 +554,18 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     __shared__ unsigned char s_pend[SKM_W];   // the window's records still to be collapsed into the buffer
     __shared__ unsigned s_new, s_tot_new;
     __shared__ u64 s_staged, s_drained;   // records staged, distinct records drained (PGB200_SKM_STATS)
+    __shared__ u32 s_coll, s_ad_n;        // collapse the next bucket's records; buckets since the auto mode last decided
+    __shared__ u64 s_ad_staged, s_ad_drained;   // s_staged, s_drained when it did
     __shared__ SweepTally s_sw;   // the fused sweeps (a.sweep)
+#ifdef SKM_PHASE_CLOCKS
+    __shared__ u64 s_wall[SKM_WALL_PHASES];
+    __shared__ long long s_wall_last;
+    const long long t_kernel = clock64();
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < SKM_WALL_PHASES; i++) s_wall[i] = 0;
+        s_wall_last = t_kernel;
+    }
+#endif
     SmemTable<NW, SKM_SLOTS, SKM_SOFT_LIMIT, unsigned short> st{s_dyn, s_dyn + NW * SKM_SLOTS, s_dyn + (NW + 1) * SKM_SLOTS, s_list, &s_count};
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const unsigned lane_le = 0xffffffffu >> (31 - lane);
@@ -532,6 +580,10 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         s_nbuf = 0;
         s_staged = 0;
         s_drained = 0;
+        s_coll = a.collapse != SKM_COLLAPSE_OFF;
+        s_ad_n = 0;
+        s_ad_staged = 0;
+        s_ad_drained = 0;
         mbar_init(&s_bar[0], 1);
         mbar_init(&s_bar[1], 1);
     }
@@ -563,8 +615,9 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     cur.cum = cta_exclusive_scan(cur.cnt, s_warp, R_cur);
     unsigned half = 0, phase = 0;        // stage half of the current window; bit h: parity of half h's next completion
     __syncthreads();                     // the mbarriers are initialised
-    if (pos < a.n_list) skm_stage_window<RW>(s_stage, &s_bar[0], my_recs, cur, R_cur, 0);
+    if (pos < a.n_list) skm_stage_window<RW, SKM_W>(s_stage, &s_bar[0], my_recs, cur, R_cur, 0);
     for (; pos < a.n_list; pos += gridDim.x) {
+        SKM_WALL(6);
         __syncthreads();   // previous bucket fully flushed (and the empty table visible on the first trip)
         u32 R_nxt;
         nxt.cum = cta_exclusive_scan(nxt.cnt, s_warp, R_nxt);
@@ -600,6 +653,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             s_defer = defer ? 1u : 0u;
         }
         __syncthreads();
+        SKM_WALL(0);
         const bool run = !s_defer && R > 0;
         // ---- drain: the nb buffered records -> their k-mer instances -> the shared-memory table; the buffer is empty again
         auto drain = [&](u32 nb) {
@@ -620,6 +674,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             if (tid == 0) s_P[nb] = I;
             __syncthreads();
             SKM_ACC(1, t_pre);
+            SKM_WALL(3);
             // ---- the warps: contiguous slices of the buffer's instances, 32 consecutive instances per step
             const u32 steps = (I + 31) / 32, per = (steps + WARPS - 1) / WARPS;
             const u32 q_end = min(I, (wid + 1) * per * 32);
@@ -675,18 +730,22 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
                 __syncwarp();
             }
             __syncthreads();   // the buffer, its counts, P and rv are free again
-            for (int i = tid; i < SKM_DEDUP_SLOTS; i += SKM_APPLY_THREADS) s_dd[i] = SKM_DD_EMPTY;
+            if (!COPY_PATH || s_coll)
+                for (int i = tid; i < SKM_DEDUP_SLOTS; i += SKM_APPLY_THREADS) s_dd[i] = SKM_DD_EMPTY;
             if (tid == 0) { s_nbuf = 0; s_drained += nb; }
             __syncthreads();
+            SKM_WALL(4);
         };
         // ---- the windows of the bucket (a deferred or empty bucket still retires the window queued for it)
         for (u32 w = 0;; w++) {
             const bool more = run && (w + 1) * (u32)SKM_W < R;
-            if (more) skm_stage_window<RW>(s_stage + (half ^ 1) * SKM_W * RW, &s_bar[half ^ 1], my_recs, cur, R, w + 1);
-            else if (pos + gridDim.x < a.n_list) skm_stage_window<RW>(s_stage + (half ^ 1) * SKM_W * RW, &s_bar[half ^ 1], my_recs, nxt, R_nxt, 0);
+            if (more) skm_stage_window<RW, SKM_W>(s_stage + (half ^ 1) * SKM_W * RW, &s_bar[half ^ 1], my_recs, cur, R, w + 1);
+            else if (pos + gridDim.x < a.n_list) skm_stage_window<RW, SKM_W>(s_stage + (half ^ 1) * SKM_W * RW, &s_bar[half ^ 1], my_recs, nxt, R_nxt, 0);
+            SKM_WALL(6);
             SKM_T0(t_wait);
             mbar_wait(&s_bar[half], (phase >> half) & 1u);
             SKM_ACC(0, t_wait);
+            SKM_WALL(1);
             phase ^= 1u << half;
             if (run) {
                 const u64* stg = s_stage + half * SKM_W * RW;
@@ -695,12 +754,27 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
                 if (tid < SKM_W) s_pend[tid] = (u32)tid < nrec;   // (in shared memory: nothing of the window stays in registers over a drain)
                 for (;;) {
                     SKM_T0(t_dd);
-                    if (tid < SKM_W && s_pend[tid]) s_pend[tid] = skm_dedup_insert<NW>(stg + tid * RW, s_buf, s_cnt, s_dd, &s_nbuf);
-                    __syncthreads();
+                    u32 nb;
+                    if (!COPY_PATH || s_coll) {   // (read from shared memory, not held in a register over the drains; it only changes after a flush)
+                        if (tid < SKM_W && s_pend[tid]) s_pend[tid] = skm_dedup_insert<NW>(stg + tid * RW, s_buf, s_cnt, s_dd, &s_nbuf);
+                        __syncthreads();
+                        nb = s_nbuf;
+                    } else {
+                        // Records that hardly repeat: the window is copied into the buffer with count 1, no dedup table.  Every window
+                        // but a bucket's last is full, so window w goes to buffer position (w mod C/W) * W, and a full buffer is drained.
+                        const u32 at = w % (u32)(C / SKM_W) * (u32)SKM_W;
+                        if (tid < SKM_W && s_pend[tid]) {
+#pragma unroll
+                            for (int i = 0; i < RW; i++) s_buf[(at + tid) * RW + i] = stg[tid * RW + i];
+                            s_cnt[at + tid] = 1;
+                        }
+                        __syncthreads();
+                        nb = at + min(R - w * (u32)SKM_W, (u32)SKM_W);
+                    }
                     SKM_ACC(6, t_dd);
-                    const u32 nb = s_nbuf;
+                    SKM_WALL(2);
                     const bool full = nb > (u32)C;
-                    if (!full && (more || nb == 0)) break;
+                    if (!full && ((more && (!COPY_PATH || s_coll || nb < (u32)C)) || nb == 0)) break;
                     drain(min(nb, (u32)C));   // full (the records that found no room go into the emptied buffer), or the bucket's end
                     if (!full) break;
                 }
@@ -734,9 +808,17 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         if (my_new) atomicAdd(&s_new, my_new);
         __syncthreads();
         SKM_ACC(5, t_flush);
+        SKM_WALL(5);
         if (tid == 0) {
             credit += (u64)R * SKM_MAX_RUN - (u64)s_new;   // what the bound over-reserved stays with the CTA
             s_tot_new += s_new;
+            if (COPY_PATH && a.collapse == SKM_COLLAPSE_AUTO && ++s_ad_n == (s_coll ? SKM_AUTO_PROBE : SKM_AUTO_SKIP)) {
+                // collapsing: go on while the distinct share of the records is at most the threshold; not collapsing: measure again
+                s_coll = !s_coll || (s_drained - s_ad_drained) * SKM_AUTO_DEN <= (s_staged - s_ad_staged) * SKM_AUTO_NUM;
+                s_ad_n = 0;
+                s_ad_staged = s_staged;
+                s_ad_drained = s_drained;
+            }
         }
     }
     __syncthreads();
@@ -749,14 +831,20 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     }
 #ifdef SKM_PHASE_CLOCKS
     for (int i = 0; i < SKM_PHASES; i++) atomicAdd(&g_skm_phase_clk[i], (unsigned long long)clk[i]);
+    SKM_WALL(6);
+    if (tid == 0) {
+        for (int i = 0; i < SKM_WALL_PHASES; i++) atomicAdd(&g_skm_wall_clk[i], (unsigned long long)s_wall[i]);
+        atomicAdd(&g_skm_wall_clk[SKM_WALL_PHASES], (unsigned long long)(clock64() - t_kernel));
+        atomicAdd(&g_skm_wall_clk[SKM_WALL_PHASES + 1], 1ull);
+    }
 #endif
 }
 
 // ------------------------------------------------------------------------------------------------ host side
 template <int NW>
 static constexpr size_t skm_apply_smem() {
-    return ((size_t)(NW + 2) * SKM_SLOTS + 2 * SKM_W * (NW + 2) + SKM_BUF_RECS * (NW + 2) + SKM_BUF_RECS * (NW + 1)) * sizeof(u64) +
-           (size_t)SKM_SLOTS * sizeof(unsigned short) + (2 * SKM_BUF_RECS + 1 + SKM_DEDUP_SLOTS) * sizeof(u32);
+    return ((size_t)(NW + 2) * SKM_SLOTS + 2 * skm_w<NW>() * (NW + 2) + SKM_BUF_RECS * (NW + 2) + SKM_BUF_RECS * (NW + 1)) * sizeof(u64) +
+           (size_t)SKM_SLOTS * sizeof(unsigned short) + (2 * SKM_BUF_RECS + 1 + skm_dd_slots<NW>()) * sizeof(u32);
 }
 // An aggregation launch keeps the keys the table is committed to under this share of its capacity (buckets beyond it are deferred),
 // and the growth before their re-run leaves this much HBM free
@@ -1051,6 +1139,12 @@ void EngineT<NW>::skm_launch_apply(const u32* list, u32 n_list, u32* deferred_ou
     aa.hist = hist_buf_.template as<u64>();
     aa.spill_list = spill_list_.template as<u64>();
     aa.spill_cap = SPILL_CAP;
+    aa.collapse = SKM_COLLAPSE_AUTO;
+    if (const char* e = getenv("PGB200_SKM_COLLAPSE")) {
+        if (!strcmp(e, "off")) aa.collapse = SKM_COLLAPSE_OFF;
+        else if (!strcmp(e, "on")) aa.collapse = SKM_COLLAPSE_ON;
+        else if (strcmp(e, "auto")) throw std::runtime_error("pgb200: PGB200_SKM_COLLAPSE must be auto, on or off");
+    }
     int per_sm = 0;
     PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_skm_apply<NW>, SKM_APPLY_THREADS, skm_apply_smem<NW>()));
     if (per_sm < 1) per_sm = 1;
@@ -1135,6 +1229,15 @@ void EngineT<NW>::skm_flush_complete() {
         fprintf(stderr, "[pgb200] aggregation phase clocks (thread-cycles, %% of %.3g): stage wait %.1f, instance build %.1f, find/claim %.1f, apply %.1f, "
                         "spill %.1f, flush %.1f, dedup %.1f\n", (double)tot, 100.0 * c[0] / tot, 100.0 * c[1] / tot, 100.0 * c[2] / tot, 100.0 * c[3] / tot,
                 100.0 * c[4] / tot, 100.0 * c[5] / tot, 100.0 * c[6] / tot);
+        unsigned long long wl[SKM_WALL_PHASES + 2], wzero[SKM_WALL_PHASES + 2] = {}, wsum = 0;
+        PG_CUDA(cudaMemcpyFromSymbol(wl, g_skm_wall_clk, sizeof(wl)));
+        PG_CUDA(cudaMemcpyToSymbol(g_skm_wall_clk, wzero, sizeof(wzero)));
+        for (int i = 0; i < SKM_WALL_PHASES; i++) wsum += wl[i];
+        const double ctas = wl[SKM_WALL_PHASES + 1] ? (double)wl[SKM_WALL_PHASES + 1] : 1.0, kern = wl[SKM_WALL_PHASES] ? (double)wl[SKM_WALL_PHASES] : 1.0;
+        fprintf(stderr, "[pgb200] aggregation wall split (thread 0 of each of %.0f CTAs, %% of %.4g cycles per CTA): top of bucket %.1f, stage wait %.1f, "
+                        "dedup/copy %.1f, drain pre-pass %.1f, drain steps %.1f, flush %.1f, other %.1f; phases sum to %.4f of kernel end - start\n",
+                ctas, kern / ctas, 100.0 * wl[0] / kern, 100.0 * wl[1] / kern, 100.0 * wl[2] / kern, 100.0 * wl[3] / kern, 100.0 * wl[4] / kern,
+                100.0 * wl[5] / kern, 100.0 * wl[6] / kern, (double)wsum / kern);
     }
 #endif
 }
