@@ -3,8 +3,11 @@
 // Replaces (reference file:line, standardPregraph/):
 //   prlContig2nodes / chopKmer4read / singleKmer   prlHashCtg.c:129-155, 185-256, 325-467   -> k_map_contigs
 //   chopKmer4read / searchKmer / parse1read        prlRead2Ctg.c:153-361                    -> k_map_reads
-// Text decoding is pass 1's (decode_lines / decode_records, decode.cu), or the fgets reader (reader.cu) that reads wrapped records
-// as the reference's map stage does; the host (map_stage.cpp) parses .contig, builds the batches and restates recordAlldgn.
+// Text decoding is pass 1's (decode_lines / decode_records, decode.cu, then k_pack_reads), or the fgets reader (reader.cu) that reads
+// wrapped records as the reference's map stage does; the host (map_stage.cpp) parses .contig, builds the batches and restates
+// recordAlldgn.  Both readers return, and both read kernels take, one layout: each read packed 2 bits per base at its own length,
+// ceil(len / 32) words, located by word offsets.  k_map_contigs, k_map_reads and k_map_long share one k-mer step (kmer_at: roll,
+// canonical; read_hit adds the lookup) and the two read kernels one placement (map_hit).
 //
 // Contig table.  Every canonical k-mer of every kept contig is inserted into a Table<NW> with the claim protocol of pass 1.  The
 // claimer stores the payload {contig id (bits 0..31), position mod 2^24 (bits 32..55, the reference's 24-bit r_links field), twin
@@ -26,11 +29,12 @@
 // complement pair and roll from there, look each k-mer up with map_lookup and write the hit to the span as k_map_reads does.  Each
 // hit is also counted in a shared-memory group table keyed by contig id; parse1read's result is a function of the groups' (count,
 // first index) alone, and the table stays exact past its size by grouping the leftover ids in further rounds (map_group.cuh has
-// the argument).  The reads are stored at their own packed length, located by word offsets.
+// the argument).
 #include "engine_impl.cuh"
 #include "map.h"
 #include "map_group.cuh"
 #include "reader.cuh"
+#include "scan.cuh"
 #include <algorithm>
 #include <cstdlib>
 
@@ -82,24 +86,30 @@ PG_D Kmer<NW> kcanon(const Kmer<NW>& f, const Kmer<NW>& rc, bool smaller) {
     return c;
 }
 
+// The canonical form of k-mer j of the bases at w (bases b + j .. b + j + K - 1).  k holds k-mer j - 1 and is rolled on by one base,
+// except at the first k-mer j0 of a loop, which first_kmer built.  *smaller: the forward k-mer is the smaller (isSmaller).
+template <int NW>
+PG_D Kmer<NW> kmer_at(const u64* __restrict__ w, u32 b, u32 j, u32 j0, KPair<NW>& k, const KParams<NW>& kp, bool* smaller) {
+    if (j > j0) {
+        const u32 p = b + j + kp.K - 1;
+        const unsigned c = (unsigned)(w[p >> 5] >> (2 * (p & 31))) & 3u;
+        k.f = knext(k.f, c, kp);
+        k.rc = kprev_reg(k.rc, c ^ 2u, kp);
+    }
+    *smaller = kless(k.f, k.rc);
+    return kcanon(k.f, k.rc, *smaller);
+}
+
 template <int NW>
 __global__ void __launch_bounds__(256) k_map_contigs(Table<NW> t, KParams<NW> kp, const u64* __restrict__ bases, const CtgSeg* __restrict__ segs, u64 n_seg,
                                                      u64* __restrict__ n_claimed) {
     u64 mine = 0;
     for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += (u64)gridDim.x * blockDim.x) {
         const CtgSeg g = segs[s];
-        const KPair<NW> k0 = first_kmer(bases, g.base, kp);
-        Kmer<NW> f = k0.f, rc = k0.rc;
+        KPair<NW> k = first_kmer(bases, g.base, kp);
         for (u32 j = 0; j < g.n; j++) {
-            if (j) {
-                const u64 p = g.base + j + kp.K - 1;
-                const unsigned c = (unsigned)(bases[p >> 5] >> (2 * (p & 31))) & 3u;
-                f = knext(f, c, kp);
-                rc = kprev_reg(rc, c ^ 2u, kp);
-            }
-            const bool smaller = kless(f, rc);
-            bool claimed;
-            const u64 idx = table_find_or_claim(t, kcanon(f, rc, smaller), &claimed);
+            bool smaller, claimed;
+            const u64 idx = table_find_or_claim(t, kmer_at(bases + (g.base >> 5), (u32)(g.base & 31), j, 0u, k, kp, &smaller), &claimed);
             Slot<NW>* sl = t.slots + idx;
             if (claimed) { sl->payload = (u64)g.ctg_id | ((u64)((g.pos0 + j) & 0xFFFFFFu) << 32) | ((u64)(smaller ? 0 : 1) << 56); mine++; }
             atomicAdd(&sl->aux, 1ull);
@@ -127,30 +137,41 @@ PG_D u64 map_lookup(const Table<NW>& t, const Kmer<NW>& k) {
     }
 }
 
+// the span entry of read k-mer j (kmer_at's rolling): its contig's payload | HIT_VALID with isSmaller at HIT_SMALLER_SHIFT, or 0
 template <int NW>
-__global__ void __launch_bounds__(128) k_map_reads(Table<NW> t, KParams<NW> kp, const u64* __restrict__ words, const u32* __restrict__ lens,
-                                                   const u64* __restrict__ kofs, u64 n_reads, int W64, int alignlen, u64* __restrict__ hits,
-                                                   MapHit* __restrict__ out) {
+PG_D u64 read_hit(const Table<NW>& t, const u64* __restrict__ w, u32 j, u32 j0, KPair<NW>& k, const KParams<NW>& kp) {
+    bool smaller;
+    const u64 v = map_lookup(t, kmer_at(w, 0u, j, j0, k, kp, &smaller));
+    return v ? v | ((u64)smaller << HIT_SMALLER_SHIFT) : 0ull;
+}
+
+// parse1read's placement from the winning group's first hit `best`, at index best_j of the read
+PG_D MapHit map_hit(u64 best, u32 best_j, u32 counter2) {
+    const unsigned twin = (unsigned)(best >> 56) & 3u, smaller = (unsigned)(best >> HIT_SMALLER_SHIFT) & 1u;
+    return MapHit{(u32)best, (int)((best >> 32) & 0xFFFFFFu), (int)best_j + 1,
+                  MAP_PLACED | (twin == smaller ? MAP_MINUS : 0u) | (counter2 > 1 ? MAP_FOOTPRINT : 0u)};
+}
+
+// A read's two offsets in one word, so that a thread holds one value for both (k_map_reads keeps 32 registers at NW = 2): its first
+// word in the batch's words (bits 32..63) and its first hit in the batch's span (bits 0..31).  A batch holds 100 M / (L - K + 1) reads
+// of at most L bases, L >= K: at most 100 M k-mers and 4 x 100 M words, so both fit (map_batch checks).
+PG_D const u64* read_words(const u64* words, u64 o) { return words + (o >> 32); }
+PG_D u64* read_hits(u64* hits, u64 o) { return hits + (u32)o; }
+
+// one thread per read (grid-stride over the batch); read r's words and hits are at ofs[r]
+template <int NW>
+__global__ void __launch_bounds__(128) k_map_reads(Table<NW> t, KParams<NW> kp, const u64* __restrict__ words, const u64* __restrict__ ofs,
+                                                   const u32* __restrict__ lens, u64 n_reads, int alignlen,
+                                                   u64* __restrict__ hits, MapHit* __restrict__ out) {
     const int K = kp.K;
     for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < n_reads; r += (u64)gridDim.x * blockDim.x) {
         const int len = (int)lens[r];
-        const u64* w = words + r * (u64)W64;
-        u64* h = hits + kofs[r];
+        const u64* w = read_words(words, ofs[r]);
+        u64* h = read_hits(hits, ofs[r]);
         const int nk = len >= K + 1 ? len - K + 1 : 0;   // chopKmer4read returns early below K+1 (the span is empty)
         if (nk > 0) {
-            const KPair<NW> k0 = first_kmer(w, 0, kp);
-            Kmer<NW> f = k0.f, rc = k0.rc;
-            for (int j = 0; j < nk; j++) {
-                if (j) {
-                    const int p = j + K - 1;
-                    const unsigned c = (unsigned)(w[p >> 5] >> (2 * (p & 31))) & 3u;
-                    f = knext(f, c, kp);
-                    rc = kprev_reg(rc, c ^ 2u, kp);
-                }
-                const bool smaller = kless(f, rc);
-                const u64 v = map_lookup(t, kcanon(f, rc, smaller));
-                h[j] = v ? v | ((u64)smaller << HIT_SMALLER_SHIFT) : 0ull;
-            }
+            KPair<NW> k = first_kmer(w, 0, kp);
+            for (int j = 0; j < nk; j++) h[j] = read_hit(t, w, (u32)j, 0u, k, kp);
         }
         // parse1read
         const int alldgn = len > alignlen ? alignlen : len;
@@ -170,22 +191,14 @@ __global__ void __launch_bounds__(128) k_map_reads(Table<NW> t, KParams<NW> kp, 
             counter++;
             if (flag > max_occ) { best_j = j; max_occ = flag; best = v; }
         }
-        MapHit o{0u, 0, 0, 0u};
-        if (counter) {
-            const unsigned twin = (unsigned)(best >> 56) & 3u, smaller = (unsigned)(best >> HIT_SMALLER_SHIFT) & 1u;
-            o.ctg = (u32)best;
-            o.node_pos = (int)((best >> 32) & 0xFFFFFFu);
-            o.i = best_j + 1;
-            o.flags = MAP_PLACED | (twin == smaller ? MAP_MINUS : 0u) | (counter2 > 1 ? MAP_FOOTPRINT : 0u);
-        }
-        out[r] = o;
+        out[r] = counter ? map_hit(best, (u32)best_j, (u32)counter2) : MapHit{0u, 0, 0, 0u};
     }
 }
 
-// one CTA per read (grid-stride over the batch); read r is words[wofs[r] ...], its hits go to hits[kofs[r] ...]
+// one CTA per read (grid-stride over the batch); read r's words and hits are at ofs[r]
 template <int NW>
-__global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KParams<NW> kp, const u64* __restrict__ words, const u64* __restrict__ wofs,
-                                                               const u32* __restrict__ lens, const u64* __restrict__ kofs, u64 n_reads, int alignlen,
+__global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KParams<NW> kp, const u64* __restrict__ words, const u64* __restrict__ ofs,
+                                                               const u32* __restrict__ lens, u64 n_reads, int alignlen,
                                                                u32 n_groups, u64* __restrict__ hits, MapHit* __restrict__ out) {
     __shared__ u32 s_id[MAP_GROUPS], s_cnt[MAP_GROUPS], s_first[MAP_GROUPS];
     __shared__ GroupAcc s_acc;
@@ -194,8 +207,8 @@ __global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KPar
     const GroupTab g{s_id, s_cnt, s_first, n_groups};
     for (u64 r = blockIdx.x; r < n_reads; r += gridDim.x) {
         const int len = (int)lens[r];
-        const u64* w = words + wofs[r];
-        u64* h = hits + kofs[r];
+        const u64* w = read_words(words, ofs[r]);
+        u64* h = read_hits(hits, ofs[r]);
         const u32 nk = len >= K + 1 ? (u32)(len - K + 1) : 0u;   // chopKmer4read returns early below K+1 (the span is empty)
         group_clear(g, tid, nthr);
         if (tid == 0) { s_acc = GroupAcc{0u, 0u, 0ull}; s_pending = 0; }
@@ -204,18 +217,10 @@ __global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KPar
         const u32 per = max((u32)MAP_SEG, (nk + nthr - 1) / nthr);
         const u32 j0 = min(nk, (u32)tid * per), j1 = min(nk, j0 + per);
         if (j0 < j1) {
-            const KPair<NW> k0 = first_kmer(w, j0, kp);
-            Kmer<NW> f = k0.f, rc = k0.rc;
+            KPair<NW> k = first_kmer(w, j0, kp);
             for (u32 j = j0; j < j1; j++) {
-                if (j > j0) {
-                    const u32 p = j + K - 1;
-                    const unsigned c = (unsigned)(w[p >> 5] >> (2 * (p & 31))) & 3u;
-                    f = knext(f, c, kp);
-                    rc = kprev_reg(rc, c ^ 2u, kp);
-                }
-                const bool smaller = kless(f, rc);
-                const u64 v = map_lookup(t, kcanon(f, rc, smaller));
-                h[j] = v ? v | ((u64)smaller << HIT_SMALLER_SHIFT) : 0ull;
+                const u64 v = read_hit(t, w, j, j0, k, kp);
+                h[j] = v;
                 if (v) group_add_hit(h, j, g, &s_pending);
             }
         }
@@ -235,38 +240,35 @@ __global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KPar
         }
         if (tid == 0) {
             const GroupAcc a = s_acc;
-            MapHit o{0u, 0, 0, 0u};
-            if (a.counter) {
-                const u32 bj = group_best_j(a);
-                const u64 best = h[bj];
-                const unsigned twin = (unsigned)(best >> 56) & 3u, smaller = (unsigned)(best >> HIT_SMALLER_SHIFT) & 1u;
-                o.ctg = (u32)best;
-                o.node_pos = (int)((best >> 32) & 0xFFFFFFu);
-                o.i = (int)bj + 1;
-                o.flags = MAP_PLACED | (twin == smaller ? MAP_MINUS : 0u) | (a.counter2 > 1 ? MAP_FOOTPRINT : 0u);
-            }
-            out[r] = o;
+            const u32 bj = group_best_j(a);
+            out[r] = a.counter ? map_hit(h[bj], bj, a.counter2) : MapHit{0u, 0, 0, 0u};
         }
         __syncthreads();   // s_acc is read before the next read resets it
     }
 }
 
-// strided decode output (stride words per read) -> packed at each read's own length, read r at ofs[r]
+// words of a read packed at its own length
+struct WordsOfLen {
+    const u32* lens;
+    __device__ u64 operator()(u64 i) const { return (lens[i] + 31u) / 32u; }
+};
+
+// strided decode output (stride words per read) -> packed at each read's own length, read r at ofs[r]; one thread per input word
 __global__ void __launch_bounds__(256) k_pack_reads(const u64* __restrict__ in, int stride, const u32* __restrict__ lens, const u64* __restrict__ ofs,
                                                     u64 n, u64* __restrict__ packed) {
-    const int lane = threadIdx.x & 31;
-    for (u64 r = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += ((u64)gridDim.x * blockDim.x) >> 5) {
-        const u32 nw = (lens[r] + 31) / 32;
-        for (u32 i = lane; i < nw; i += 32) packed[ofs[r] + i] = in[r * (u64)stride + i];
+    const u64 total = n * (u64)stride;
+    for (u64 idx = (u64)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (u64)gridDim.x * blockDim.x) {
+        const u64 r = idx / (unsigned)stride;
+        const u32 w = (u32)(idx - r * (unsigned)stride);
+        if (w < (lens[r] + 31) / 32) packed[ofs[r] + w] = in[idx];
     }
 }
 
 template <int NW>
 class MapEngineT : public IMapEngine {
 public:
-    MapEngineT(int K, int device, int max_rd_len) : K_(K), device_(device) {
+    MapEngineT(int K, int device) : K_(K), device_(device) {
         kp_ = make_kparams<NW>(K);
-        W64_ = std::max(1, (max_rd_len + 31) / 32);
         PG_CUDA(cudaSetDevice(device));
         PG_CUDA(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device));
         PG_CUDA(cudaStreamCreateWithFlags(&st_.h, cudaStreamNonBlocking));
@@ -276,7 +278,6 @@ public:
         PG_CUDA(cudaMemsetAsync(cnt_.p, 0, C_COUNT * sizeof(u64), st_));
     }
     ~MapEngineT() override { if (st_) cudaStreamSynchronize(st_); }
-    int words_per_read() const override { return W64_; }
 
     void hash_contigs(const u64* packed, u64 n_bases, const u64* ctg_off, const u32* ctg_id, u64 n_ctg, u64* distinct) override {
         std::vector<CtgSeg> segs;
@@ -310,8 +311,7 @@ public:
         *distinct = h_cnt_[C_DISTINCT];
     }
 
-    void decode_text(const char* text, size_t nbytes, int fastq, int reverse, int maxlen, int stride, std::vector<u64>* words,
-                     std::vector<u32>* lens) override {
+    void decode_text(const char* text, size_t nbytes, int fastq, int reverse, int maxlen, std::vector<u64>* words, std::vector<u32>* lens) override {
         if (nbytes == 0) return;
         if (nbytes >= (1ull << 32)) throw std::runtime_error("pgb200: a text chunk must be smaller than 4 GiB (feed it in pieces)");
         PG_CUDA(cudaSetDevice(device_));
@@ -322,37 +322,32 @@ public:
         const DecodeLines L = decode_lines(d_text, nbytes, fastq, n_sm_, scan_buf_, line_buf_, cnt_.as<u64>(), h_cnt_, st_);
         if (L.n_rec == 0) return;
         const u64 n = L.n_rec;
-        const int S = stride > 0 ? stride : std::max(1, (maxlen + 31) / 32);   // the decode's stride: room for maxlen bases
+        const int S = std::max(1, (maxlen + 31) / 32);   // the decode's stride: room for maxlen bases
         read_words_.ensure(n * S * sizeof(u64));
         read_lens_.ensure(n * sizeof(u32));
         decode_records(d_text, nbytes, L, maxlen, reverse, K_, S, n_sm_, read_words_.as<u64>(), read_lens_.as<u32>(), cnt_.as<u64>(), st_);
-        if (stride > 0) PG_CUDA(cudaEventRecord(ev_[1], st_));
+        // each read packed at its own length, ceil(len / 32) words, at the exclusive scan of those counts; pack_ofs_[n]: the total
+        pack_ofs_.ensure((n + 1) * sizeof(u64));
+        pack_scan_.ensure(scan_scratch_elems(n) * sizeof(u64));
+        pack_words_.ensure(n * S * sizeof(u64));
+        u64* ofs = pack_ofs_.as<u64>();
+        device_scan(WordsOfLen{read_lens_.as<u32>()}, ScanU64Out{ofs}, n, pack_scan_.as<u64>(), ofs + n, st_);
+        k_pack_reads<<<(unsigned)std::min<u64>((n * S + 255) / 256, (u64)n_sm_ * 64), 256, 0, st_>>>(read_words_.as<u64>(), S, read_lens_.as<u32>(), ofs, n,
+                                                                                             pack_words_.as<u64>());
+        PG_CUDA(cudaGetLastError());
+        PG_CUDA(cudaEventRecord(ev_[1], st_));
         const size_t w0 = words->size(), l0 = lens->size();
         lens->resize(l0 + n);
         PG_CUDA(cudaMemcpyAsync(lens->data() + l0, read_lens_.p, n * sizeof(u32), cudaMemcpyDeviceToHost, st_));
         // the line index of THIS chunk flags malformed records (decode_lines checked the counters before it ran)
         PG_CUDA(cudaMemcpyAsync(h_cnt_, cnt_.p, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st_));
-        u64 n_words = n * S;
-        const u64* src = read_words_.as<u64>();
-        if (stride <= 0) {   // packed: each read at its own length, ceil(len / 32) words
-            PG_CUDA(cudaStreamSynchronize(st_));
-            check_format(h_cnt_);
-            std::vector<u64> ofs(n);
-            n_words = 0;
-            for (u64 r = 0; r < n; r++) { ofs[r] = n_words; n_words += ((*lens)[l0 + r] + 31) / 32; }
-            pack_ofs_.ensure(n * sizeof(u64));
-            pack_words_.ensure(n_words * sizeof(u64) + 8);
-            PG_CUDA(cudaMemcpyAsync(pack_ofs_.p, ofs.data(), n * sizeof(u64), cudaMemcpyHostToDevice, st_));
-            k_pack_reads<<<(unsigned)std::min<u64>((n + 7) / 8, (u64)n_sm_ * 16), 256, 0, st_>>>(src, S, read_lens_.as<u32>(), pack_ofs_.as<u64>(), n,
-                                                                                                 pack_words_.as<u64>());
-            PG_CUDA(cudaGetLastError());
-            PG_CUDA(cudaEventRecord(ev_[1], st_));
-            src = pack_words_.as<u64>();
-        }
-        words->resize(w0 + n_words);
-        PG_CUDA(cudaMemcpyAsync(words->data() + w0, src, n_words * sizeof(u64), cudaMemcpyDeviceToHost, st_));
+        PG_CUDA(cudaMemcpyAsync(h_cnt_ + C_COUNT + 1, ofs + n, sizeof(u64), cudaMemcpyDeviceToHost, st_));
         PG_CUDA(cudaStreamSynchronize(st_));
         check_format(h_cnt_);
+        const u64 n_words = h_cnt_[C_COUNT + 1];
+        words->resize(w0 + n_words);
+        PG_CUDA(cudaMemcpyAsync(words->data() + w0, pack_words_.p, n_words * sizeof(u64), cudaMemcpyDeviceToHost, st_));
+        PG_CUDA(cudaStreamSynchronize(st_));
         float ms;
         PG_CUDA(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
         ms_decode_ += ms;
@@ -374,56 +369,30 @@ public:
         return cut;
     }
 
-    void map_batch(const u64* words, const u32* lens, u64 n, int alignlen, MapHit* out) override {
+    void map_batch(const u64* words, u64 n_words, const u64* wofs, const u32* lens, u64 n, int alignlen, bool per_read_cta, MapHit* out) override {
         PG_CUDA(cudaSetDevice(device_));
-        std::vector<u64> kofs(n + 1);
+        std::vector<u64> ofs(n);   // read_words / read_hits
         u64 k = 0;
-        for (u64 r = 0; r < n; r++) { kofs[r] = k; if ((int)lens[r] >= K_ + 1) k += lens[r] - K_ + 1; }
-        kofs[n] = k;
-        batch_words_.ensure(n * W64_ * sizeof(u64));
-        batch_lens_.ensure(n * sizeof(u32) + 4);
-        batch_kofs_.ensure((n + 1) * sizeof(u64));
-        hits_.ensure(k * sizeof(u64) + 8);
-        out_.ensure(n * sizeof(MapHit) + 16);
-        PG_CUDA(cudaMemcpyAsync(batch_words_.p, words, n * W64_ * sizeof(u64), cudaMemcpyHostToDevice, st_));
-        PG_CUDA(cudaMemcpyAsync(batch_lens_.p, lens, n * sizeof(u32), cudaMemcpyHostToDevice, st_));
-        PG_CUDA(cudaMemcpyAsync(batch_kofs_.p, kofs.data(), (n + 1) * sizeof(u64), cudaMemcpyHostToDevice, st_));
-        PG_CUDA(cudaEventRecord(ev_[0], st_));
-        if (n) {
-            k_map_reads<NW><<<(unsigned)std::min<u64>((n + 127) / 128, (u64)n_sm_ * 16), 128, 0, st_>>>(tab_, kp_, batch_words_.as<u64>(), batch_lens_.as<u32>(),
-                                                                                                   batch_kofs_.as<u64>(), n, W64_, alignlen, hits_.as<u64>(),
-                                                                                                   out_.as<MapHit>());
-            PG_CUDA(cudaGetLastError());
-        }
-        PG_CUDA(cudaEventRecord(ev_[1], st_));
-        PG_CUDA(cudaMemcpyAsync(out, out_.p, n * sizeof(MapHit), cudaMemcpyDeviceToHost, st_));
-        PG_CUDA(cudaStreamSynchronize(st_));
-        float ms;
-        PG_CUDA(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
-        ms_scan_ += ms;
-    }
-
-    void map_long_batch(const u64* words, u64 n_words, const u64* wofs, const u32* lens, u64 n, int alignlen, MapHit* out) override {
-        PG_CUDA(cudaSetDevice(device_));
-        std::vector<u64> kofs(n + 1);
-        u64 k = 0;
-        for (u64 r = 0; r < n; r++) { kofs[r] = k; if ((int)lens[r] >= K_ + 1) k += lens[r] - K_ + 1; }
-        kofs[n] = k;
+        for (u64 r = 0; r < n; r++) { ofs[r] = wofs[r] << 32 | k; if ((int)lens[r] >= K_ + 1) k += lens[r] - K_ + 1; }
+        if (n_words >> 32 || k >> 32) throw std::runtime_error("pgb200: a map batch holds 2^32 words or k-mers");
         batch_words_.ensure(n_words * sizeof(u64) + 8);
-        batch_wofs_.ensure(n * sizeof(u64) + 8);
+        batch_ofs_.ensure(n * sizeof(u64) + 8);
         batch_lens_.ensure(n * sizeof(u32) + 4);
-        batch_kofs_.ensure((n + 1) * sizeof(u64));
         hits_.ensure(k * sizeof(u64) + 8);
         out_.ensure(n * sizeof(MapHit) + 16);
         PG_CUDA(cudaMemcpyAsync(batch_words_.p, words, n_words * sizeof(u64), cudaMemcpyHostToDevice, st_));
-        PG_CUDA(cudaMemcpyAsync(batch_wofs_.p, wofs, n * sizeof(u64), cudaMemcpyHostToDevice, st_));
+        PG_CUDA(cudaMemcpyAsync(batch_ofs_.p, ofs.data(), n * sizeof(u64), cudaMemcpyHostToDevice, st_));
         PG_CUDA(cudaMemcpyAsync(batch_lens_.p, lens, n * sizeof(u32), cudaMemcpyHostToDevice, st_));
-        PG_CUDA(cudaMemcpyAsync(batch_kofs_.p, kofs.data(), (n + 1) * sizeof(u64), cudaMemcpyHostToDevice, st_));
         PG_CUDA(cudaEventRecord(ev_[0], st_));
         if (n) {
-            k_map_long<NW><<<(unsigned)std::min<u64>(n, (u64)n_sm_ * 16), MAP_LONG_THREADS, 0, st_>>>(tab_, kp_, batch_words_.as<u64>(), batch_wofs_.as<u64>(),
-                                                                                                       batch_lens_.as<u32>(), batch_kofs_.as<u64>(), n, alignlen,
-                                                                                                       n_groups_, hits_.as<u64>(), out_.as<MapHit>());
+            if (per_read_cta)
+                k_map_long<NW><<<(unsigned)std::min<u64>(n, (u64)n_sm_ * 16), MAP_LONG_THREADS, 0, st_>>>(tab_, kp_, batch_words_.as<u64>(), batch_ofs_.as<u64>(),
+                                                                                                           batch_lens_.as<u32>(), n, alignlen,
+                                                                                                           n_groups_, hits_.as<u64>(), out_.as<MapHit>());
+            else
+                k_map_reads<NW><<<(unsigned)std::min<u64>((n + 127) / 128, (u64)n_sm_ * 16), 128, 0, st_>>>(tab_, kp_, batch_words_.as<u64>(), batch_ofs_.as<u64>(),
+                                                                                                       batch_lens_.as<u32>(), n, alignlen,
+                                                                                                       hits_.as<u64>(), out_.as<MapHit>());
             PG_CUDA(cudaGetLastError());
         }
         PG_CUDA(cudaEventRecord(ev_[1], st_));
@@ -431,30 +400,32 @@ public:
         PG_CUDA(cudaStreamSynchronize(st_));
         float ms;
         PG_CUDA(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
-        ms_long_ += ms;
-        lookups_long_ += k;
+        if (per_read_cta) {
+            ms_long_ += ms;
+            lookups_long_ += k;
+        } else ms_scan_ += ms;
     }
     void times(MapTimes* t) const override { *t = MapTimes{ms_hash_, ms_decode_, ms_scan_, ms_long_, lookups_long_}; }
 
 private:
-    int K_, device_, W64_ = 1, n_sm_ = 0;
+    int K_, device_, n_sm_ = 0;
     // group slots of k_map_long; PGB200_MAP_GROUPS lowers it (1..MAP_GROUPS) so that a test can force the overflow rounds
     u32 n_groups_ = getenv("PGB200_MAP_GROUPS") ? (u32)std::min<long>(std::max<long>(1, atol(getenv("PGB200_MAP_GROUPS"))), (long)MAP_GROUPS) : MAP_GROUPS;
     KParams<NW> kp_;
     Stream st_;
     Event ev_[2];
     Pinned<u64> h_cnt_;
-    DevBuf cnt_, tab_buf_, text_buf_, scan_buf_, line_buf_, read_words_, read_lens_, pack_ofs_, pack_words_, batch_words_, batch_wofs_, batch_lens_,
-        batch_kofs_, hits_, out_;
+    DevBuf cnt_, tab_buf_, text_buf_, scan_buf_, line_buf_, read_words_, read_lens_, pack_ofs_, pack_scan_, pack_words_, batch_words_, batch_ofs_,
+        batch_lens_, hits_, out_;
     Table<NW> tab_{nullptr, 0};
     FgetsReader reader_;
     double ms_hash_ = 0, ms_decode_ = 0, ms_scan_ = 0, ms_long_ = 0;
     u64 lookups_long_ = 0;
 };
 
-IMapEngine* make_map_engine(int K, int device, int max_rd_len) {
-    if (K <= 63) return new MapEngineT<2>(K, device, max_rd_len);
-    return new MapEngineT<4>(K, device, max_rd_len);
+IMapEngine* make_map_engine(int K, int device) {
+    if (K <= 63) return new MapEngineT<2>(K, device);
+    return new MapEngineT<4>(K, device);
 }
 
 }   // namespace pgb

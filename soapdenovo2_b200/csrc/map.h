@@ -31,27 +31,27 @@ struct MapTimes {
 class IMapEngine {
 public:
     virtual ~IMapEngine() {}
-    virtual int words_per_read() const = 0;   // W64: 2-bit packed words per read (LSB first), from max_rd_len
     // the contig k-mer table: bases packed 2 bits each (LSB first) into one stream, contig c = bases [ctg_off[c], ctg_off[c+1])
     virtual void hash_contigs(const u64* packed, u64 n_bases, const u64* ctg_off, const u32* ctg_id, u64 n_ctg,
                               u64* distinct) = 0;
-    // one chunk of whole FASTA/FASTQ records, each cut to maxlen bases -> its reads appended to *words and *lens: `stride` words per
-    // read (>= (maxlen + 31) / 32), or with stride 0 each read packed at its own length, ceil(len / 32) words, one after another
-    virtual void decode_text(const char* text, size_t nbytes, int fastq, int reverse, int maxlen, int stride, std::vector<u64>* words,
-                             std::vector<u32>* lens) = 0;
+    // Reads come back, and go into map_batch, packed 2 bits per base (LSB first) at their own lengths: ceil(len / 32) words each, one
+    // after another.
+    // one chunk of whole FASTA/FASTQ records (pass 1's reader: single-line FASTA, 4-line FASTQ), each cut to maxlen bases -> its reads
+    // appended to *words and *lens
+    virtual void decode_text(const char* text, size_t nbytes, int fastq, int reverse, int maxlen, std::vector<u64>* words, std::vector<u32>* lens) = 0;
     // one chunk of a FASTA/FASTQ file read as the reference's map stage reads it (readseq1by1 / read1seqfq: fgets pieces of piece_len
-    // bytes, wrapped records, the raw-length cut at `cutoff`; reader.cu) -> its reads appended packed at their own lengths, as
-    // decode_text with stride 0.  at_eof: the chunk ends the file.  Returns the byte offset where the chunk's unfinished record starts
-    // (nbytes at the end of the file): the caller prepends text[result, nbytes) to its next chunk.
+    // bytes, wrapped records, the raw-length cut at `cutoff`; reader.cu) -> its reads appended to *words and *lens.  at_eof: the chunk
+    // ends the file.  Returns the byte offset where the chunk's unfinished record starts (nbytes at the end of the file): the caller
+    // prepends text[result, nbytes) to its next chunk.
     virtual size_t read_text(const char* text, size_t nbytes, int fastq, int piece_len, int cutoff, int reverse, bool at_eof, std::vector<u64>* words,
                              std::vector<u32>* lens) = 0;
-    // one batch of reads (parse1read reads ALIGNLEN once per batch: alignlen is its value after the batch's last read)
-    virtual void map_batch(const u64* words, const u32* lens, u64 n, int alignlen, MapHit* out) = 0;
-    // the same for reads located by word offsets into words[0, n_words) -- long reads, one CTA per read (k_map_long)
-    virtual void map_long_batch(const u64* words, u64 n_words, const u64* wofs, const u32* lens, u64 n, int alignlen, MapHit* out) = 0;
+    // one batch of reads, read r at words[wofs[r] ...) within words[0, n_words) (parse1read reads ALIGNLEN once per batch: alignlen
+    // is its value after the batch's last read).  per_read_cta: one CTA per read (k_map_long, for long reads), else one thread per
+    // read (k_map_reads); their GPU times are kept apart, as ms_long and ms_scan.
+    virtual void map_batch(const u64* words, u64 n_words, const u64* wofs, const u32* lens, u64 n, int alignlen, bool per_read_cta, MapHit* out) = 0;
     virtual void times(MapTimes* t) const = 0;
 };
-IMapEngine* make_map_engine(int K, int device, int max_rd_len);   // 128-bit keys for K <= 63, else 256-bit
+IMapEngine* make_map_engine(int K, int device);   // 128-bit keys for K <= 63, else 256-bit
 
 }   // namespace pgb
 #pragma GCC visibility pop

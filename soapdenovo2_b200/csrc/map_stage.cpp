@@ -168,89 +168,62 @@ ContigInfo contig_info(const std::string& prefix) {
     return ci;
 }
 
-// The reads of one pass, in the order read1seqInLib returns them (short pass: mates interleaved, W64 words per read; long pass: each
-// read packed at its own length, at wofs[r])
+// The reads of one pass, in the order read1seqInLib returns them (short pass: mates interleaved), each packed 2 bits per base (LSB
+// first) at its own length, ceil(len / 32) words at wofs[r]; wofs[n] is the word total
 struct Reads {
     std::vector<u64> words, wofs;
     std::vector<u32> lens;
     std::vector<int> lib;   // index into MapPlan::libs / long_libs
 };
-void decode_file(IMapEngine& eng, const PlanEntry& f, int maxlen, int stride, std::vector<u64>* words, std::vector<u32>* lens) {
-    std::unique_ptr<FILE, int (*)(FILE*)> file(fopen(f.path.c_str(), "rb"), fclose);
-    if (!file) fail("Cannot open %s. Now exit to system...", f.path.c_str());
-    const size_t cap = (size_t)(getenv("PGB200_CHUNK_MB") ? atoi(getenv("PGB200_CHUNK_MB")) : 256) << 20;
-    std::vector<char> buf(cap + 16);
-    size_t have = 0;
-    bool eof = false;
-    while (!eof || have) {
-        const size_t got = eof ? 0 : fread(buf.data() + have, 1, cap - have, file.get());
-        if (got == 0) eof = true;
-        have += got;
-        if (have == 0) break;
-        size_t cut;
-        if (eof) {
-            while (have > 1 && buf[have - 1] == '\n' && buf[have - 2] == '\n') have--;
-            if (have == 1 && buf[0] == '\n') have = 0;
-            if (have == 0) break;
-            cut = have;
-        } else {
-            cut = last_record_start(buf.data(), have, f.fastq);
-            if (cut == 0 && have == cap) fail("pgb200: a single record exceeds the %zu MB chunk", cap >> 20);
-            if (cut == 0) continue;
-        }
-        try { eng.decode_text(buf.data(), cut, f.fastq, f.reverse, maxlen, stride, words, lens); }
-        catch (const std::exception& ex) { fail("readseqInLib return error! please make sure input file is correct fastq/fasta file \n(%s)", ex.what()); }
-        memmove(buf.data(), buf.data() + cut, have - cut);
-        have -= cut;
-    }
-}
 
-// The same with the fgets reader (reader.cu), which reads wrapped records as readseq1by1 / read1seqfq do: the GPU reports where each
-// chunk's unfinished record starts, and the bytes from there are carried into the next chunk.  The reads arrive packed at their own
-// lengths and are laid out `stride` words apart when stride > 0.
-void read_file_fgets(IMapEngine& eng, const PlanEntry& f, int piece_len, int maxlen, int stride, std::vector<u64>* words, std::vector<u32>* lens) {
+// One file's reads, appended to *words / *lens, each cut to maxlen bases.  The file is read in PGB200_CHUNK_MB chunks cut at a record
+// boundary, the rest carried into the next chunk.  fgets_piece == 0: pass 1's reader (decode_text: single-line FASTA, 4-line FASTQ),
+// cut at the chunk's last record start, trailing blank lines dropped at the end of the file.  Otherwise the fgets reader (read_text,
+// reader.cu), which reads wrapped records as readseq1by1 / read1seqfq do, in fgets pieces of fgets_piece bytes, and finds the cut.
+void read_file(IMapEngine& eng, const PlanEntry& f, int maxlen, int fgets_piece, std::vector<u64>* words, std::vector<u32>* lens) {
     std::unique_ptr<FILE, int (*)(FILE*)> file(fopen(f.path.c_str(), "rb"), fclose);
     if (!file) fail("Cannot open %s. Now exit to system...", f.path.c_str());
     const size_t cap = (size_t)(getenv("PGB200_CHUNK_MB") ? atoi(getenv("PGB200_CHUNK_MB")) : 256) << 20;
     std::vector<char> buf(cap + 16);
-    std::vector<u64> packed;
-    const size_t l0 = lens->size();
     size_t have = 0;
     bool eof = false;
     for (;;) {
-        if (!eof && have < cap) {
-            have += fread(buf.data() + have, 1, cap - have, file.get());
-            eof = feof(file.get()) != 0;
+        if (!eof) {
+            const size_t got = fread(buf.data() + have, 1, cap - have, file.get());
+            have += got;
+            eof = fgets_piece ? feof(file.get()) != 0 : got == 0;   // pass 1's reader sees the end only in a read that finds nothing
             if (!eof && ferror(file.get())) fail("pgb200: read error on %s", f.path.c_str());
         }
         if (have == 0 && eof) break;
         size_t cut;
-        try { cut = eng.read_text(buf.data(), have, f.fastq, piece_len, maxlen, f.reverse, eof, stride > 0 ? &packed : words, lens); }
-        catch (const std::exception& ex) { fail("%s (%s)", ex.what(), f.path.c_str()); }
+        try {
+            if (fgets_piece) cut = eng.read_text(buf.data(), have, f.fastq, fgets_piece, maxlen, f.reverse, eof, words, lens);
+            else {
+                if (eof) {
+                    while (have > 1 && buf[have - 1] == '\n' && buf[have - 2] == '\n') have--;
+                    if (have == 1 && buf[0] == '\n') have = 0;
+                }
+                cut = eof ? have : last_record_start(buf.data(), have, f.fastq);
+                eng.decode_text(buf.data(), cut, f.fastq, f.reverse, maxlen, words, lens);
+            }
+        } catch (const std::exception& ex) {
+            if (fgets_piece) fail("%s (%s)", ex.what(), f.path.c_str());
+            fail("readseqInLib return error! please make sure input file is correct fastq/fasta file \n(%s)", ex.what());
+        }
         if (eof) break;
         if (cut == 0 && have == cap) fail("pgb200: a single record exceeds the %zu MB chunk", cap >> 20);
         memmove(buf.data(), buf.data() + cut, have - cut);
         have -= cut;
     }
-    if (stride > 0) {
-        u64 o = 0;
-        for (size_t r = l0; r < lens->size(); r++) {
-            const u64 n = ((*lens)[r] + 31) / 32;
-            const size_t w0 = words->size();
-            words->resize(w0 + stride, 0);
-            std::copy(packed.begin() + o, packed.begin() + o + n, words->begin() + w0);
-            o += n;
-        }
-    }
 }
 
 // One pass's reads, decoded before anything is written: every refusal comes before the first output file.  The stderr lines the
 // reference prints while it reads go to *log, to be printed where the pass prints them.  A read longer than `room` would run past
-// the reference's seqBuffer (allocated for `room` bases): no output is defined for it, so it is refused.  Each file is decoded
-// with one base of slack past `room` so that such a read shows.  fgets_gstr < 0: pass 1's reader (single-line FASTA, 4-line FASTQ);
+// the reference's seqBuffer (allocated for `room` bases): no output is defined for it, so it is refused.  Each file is read with a
+// cut one base past `room` so that such a read shows.  fgets_gstr < 0: pass 1's reader (single-line FASTA, 4-line FASTQ);
 // otherwise the fgets reader, whose pieces are the cutoff long when the pass allocated gStr (fgets_gstr = 1) and gLineLen - 1 = 4999
 // bytes long when it did not (readseq1by1.c:54-66, prlRead2Ctg.c:826, 1133).
-Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pass, int room, int stride, int fgets_gstr, std::string* log) {
+Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pass, int room, int fgets_gstr, std::string* log) {
     Reads rd;
     char line[256];
     auto say = [&](const char* fmt, auto... a) { snprintf(line, sizeof line, fmt, a...); *log += line; };
@@ -262,8 +235,7 @@ Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pas
             const int maxlen = std::min(e.cut, room + 1);
             const size_t before = rd.lens.size();
             auto read_one = [&](const PlanEntry& pe, std::vector<u64>* w, std::vector<u32>* l) {
-                if (fgets_gstr < 0) decode_file(eng, pe, maxlen, stride, w, l);
-                else read_file_fgets(eng, pe, fgets_gstr ? pe.cut : 4999, maxlen, stride, w, l);
+                read_file(eng, pe, maxlen, fgets_gstr < 0 ? 0 : fgets_gstr ? pe.cut : 4999, w, l);
             };
             if (e.mate == 0) {
                 // openFileInLib names both mates before the first read; mates then alternate r1, r2, r1, r2
@@ -276,13 +248,20 @@ Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pas
                 read_one(m, &w2, &l2);
                 if (l1.size() != l2.size())
                     fail("pgb200: mate files hold different numbers of reads (%zu vs %zu): unsupported", l1.size(), l2.size());
-                rd.words.resize(rd.words.size() + 2 * w1.size());
-                u64* dst = rd.words.data() + before * stride;
+                const size_t w0 = rd.words.size();
+                rd.words.resize(w0 + w1.size() + w2.size());
+                u64* dst = rd.words.data() + w0;
+                const u64 *s1 = w1.data(), *s2 = w2.data();
+                auto copy_read = [&](const u64*& src, u32 len) {
+                    const size_t nw = (len + 31) / 32;
+                    memcpy(dst, src, nw * sizeof(u64));
+                    dst += nw;
+                    src += nw;
+                    rd.lens.push_back(len);
+                };
                 for (size_t r = 0; r < l1.size(); r++) {
-                    memcpy(dst + (2 * r) * stride, w1.data() + r * stride, stride * sizeof(u64));
-                    memcpy(dst + (2 * r + 1) * stride, w2.data() + r * stride, stride * sizeof(u64));
-                    rd.lens.push_back(l1[r]);
-                    rd.lens.push_back(l2[r]);
+                    copy_read(s1, l1[r]);
+                    copy_read(s2, l2[r]);
                 }
             } else {
                 say("Import reads from file:\n %s\n", e.path.c_str());
@@ -302,12 +281,10 @@ Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pas
                 if ((r + 1) % 100000000 == 0) say("--- %lldth reads.\n", (long long)(r + 1));
         }
     }
-    if (stride == 0) {   // packed reads: word offsets from the lengths
-        rd.wofs.resize(rd.lens.size() + 1);
-        u64 o = 0;
-        for (size_t r = 0; r < rd.lens.size(); r++) { rd.wofs[r] = o; o += (rd.lens[r] + 31) / 32; }
-        rd.wofs.back() = o;
-    }
+    rd.wofs.resize(rd.lens.size() + 1);
+    u64 o = 0;
+    for (size_t r = 0; r < rd.lens.size(); r++) { rd.wofs[r] = o; o += (rd.lens[r] + 31) / 32; }
+    rd.wofs.back() = o;
     return rd;
 }
 
@@ -315,23 +292,24 @@ template <class T> void put(std::string& s, const T& v) { s.append(reinterpret_c
 
 struct RcSeqModel {
     std::vector<unsigned char> b;
-    void tight(const u64* w, int len) {   // writeChar2tightString of every base, seq.c:81-107
+    // writeChar2tightString of every base of w (seq.c:81-107), then the len / 4 + 1 bytes the record takes from the buffer
+    void append_tight(std::string& s, const u64* w, int len) {
         for (int i = 0; i < len; i++) {
             const unsigned c = (unsigned)(w[i >> 5] >> (2 * (i & 31))) & 3u;
             unsigned char& x = b[i / 4];
             const int sh = 6 - 2 * (i % 4);
             x = (unsigned char)((x & ~(3u << sh)) | (c << sh));
         }
+        s.append(reinterpret_cast<const char*>(b.data()), (size_t)(len / 4 + 1));
     }
     // thread 0's chops of a batch of n reads leave their reverse complements here (chopKmer4read, prlRead2Ctg.c:153-187): reads
     // t = 0 (mod P) with len >= K+1, the later ones over the earlier ones
-    template <class WordsOf>
-    void chops(u64 n, int P, int K, const u32* lens, WordsOf words_of) {
+    void chops(u64 n, int P, int K, const u32* lens, const u64* W, const u64* wofs) {
         size_t covered = 0;
         for (long long t = ((long long)n - 1) / P * P; t >= 0 && covered < b.size(); t -= P) {
             const int len = (int)lens[t];
             if (len < K + 1 || (size_t)len <= covered) continue;
-            const u64* w = words_of((u64)t);
+            const u64* w = W + wofs[t];
             for (size_t i = covered; i < (size_t)len; i++) {
                 const int src = len - 1 - (int)i;
                 b[i] = (unsigned char)((((w[src >> 5] >> (2 * (src & 31))) & 3u)) ^ 2u);
@@ -380,53 +358,82 @@ void print_libs(const MapPlan& plan) {   // free_libs, lib.c:516-520
     for (size_t i = 0; i < plan.libs.size(); i++) fprintf(stderr, " [LIB] %zu, avg_ins %d, reverse %d.\n", i, plan.libs[i].avg_ins, plan.libs[i].reverse);
 }
 
-// prlLongRead2Ctg once its reads are in: batches of maxReadNum reads (from longReadLen), parse1read on the GPU (k_map_long), and
-// recordLongRead / output1read here.  Every long read has insert size 18; a read whose footprint is set goes to .longReadInGap (len,
-// contig, pos and its bases packed from this pass's own rcSeq[1], a zeroed buffer of longReadLen bytes) and, with -f, as text to
-// .RlongReadInGap.  Both are plain files.
+// The batch work both passes share: reads [b0, b0 + n) of rd, their word offsets rebased to the batch, through parse1read on the
+// GPU (k_map_long, one CTA per read, when per_read_cta; else k_map_reads), then thread 0's chops into rc (a zeroed buffer of the
+// pass's read length: ckalloc is calloc) and the placements into pl.  read(t) is the batch's read t.
+struct BatchMapper {
+    IMapEngine& eng;
+    const Reads& rd;
+    const ContigInfo& ci;
+    const int K, P;
+    const std::string& prefix;
+    std::vector<MapHit> hit;
+    Placement pl;
+    RcSeqModel rc;
+    std::vector<u64> wofs;
+    const u64* W = nullptr;
+    const u32* lens = nullptr;
+    BatchMapper(IMapEngine& eng, const Reads& rd, long long max_read_num, int read_len, const ContigInfo& ci, int K, int P, const std::string& prefix)
+        : eng(eng), rd(rd), ci(ci), K(K), P(P), prefix(prefix), hit((size_t)std::min<long long>(max_read_num, (long long)std::max<size_t>(rd.lens.size(), 1))),
+          pl(hit.size()), rc{std::vector<unsigned char>((size_t)read_len, 0)} {}
+    const u64* read(u64 t) const { return W + wofs[t]; }
+    // returns the host time at which the GPU's placements were in
+    double map(u64 b0, u64 n, int alignlen, bool per_read_cta, const char* what) {
+        const u64 w0 = rd.wofs[b0];
+        wofs.resize(n);
+        for (u64 t = 0; t < n; t++) wofs[t] = rd.wofs[b0 + t] - w0;
+        W = rd.words.data() + w0;
+        lens = rd.lens.data() + b0;
+        try { eng.map_batch(W, rd.wofs[b0 + n] - w0, wofs.data(), lens, n, alignlen, per_read_cta, hit.data()); }
+        catch (const std::exception& ex) { fail("pgb200: %s failed: %s", what, ex.what()); }
+        const double t_mapped = host_now();
+        rc.chops(n, P, K, lens, W, wofs.data());
+        pl.set(hit.data(), n, ci, K, prefix);
+        return t_mapped;
+    }
+};
+
+// The gap record of output1read / output1read_gz: len, contig, pos, then the read packed from rcSeq[1]
+void put_gap(std::string& s, RcSeqModel& rc, const u64* w, int len, int ctg, int pos) {
+    put(s, len); put(s, ctg); put(s, pos);
+    rc.append_tight(s, w, len);
+}
+// The -f text record: ">len\tctg\tpos\torien\tins\tdh\n", then the bases
+void put_text(std::string& s, const u64* w, int len, int ctg, int pos, char o, int ins, int dh) {
+    char line[128];
+    s.append(line, (size_t)snprintf(line, sizeof line, ">%d\t%d\t%d\t%c\t%d\t%d\n", len, ctg, pos, o, ins, dh));
+    for (int i = 0; i < len; i++) s.push_back("ACTG"[(w[i >> 5] >> (2 * (i & 31))) & 3]);
+    s.push_back('\n');
+}
+
+// prlLongRead2Ctg once its reads are in: batches of maxReadNum reads (from longReadLen) and recordLongRead / output1read.  Every
+// long read has insert size 18; a read whose footprint is set goes to .longReadInGap (with this pass's own rcSeq[1], of longReadLen
+// bytes) and, with -f, as text to .RlongReadInGap.  Both are plain files.
 void map_long_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, long long max_read_num, const ContigInfo& ci, int K, int P, int fill,
                     const std::string& prefix) {
     const u64 n_reads = rd.lens.size();
-    std::vector<MapHit> hit((size_t)std::min<long long>(max_read_num, (long long)std::max<u64>(n_reads, 1)));
-    Placement pl(hit.size());
-    RcSeqModel rc{std::vector<unsigned char>((size_t)plan.long_len, 0)};
+    BatchMapper bm(eng, rd, max_read_num, plan.long_len, ci, K, P, prefix);
+    const Placement& pl = bm.pl;
     std::unique_ptr<FILE, int (*)(FILE*)> f_gap(ckopen(prefix + ".longReadInGap", "wb"), fclose);
     std::unique_ptr<FILE, int (*)(FILE*)> f_txt(fill ? ckopen(prefix + ".RlongReadInGap", "w") : nullptr, fclose);
     auto put_file = [&](FILE* f, const std::string& s, const char* suffix) {
         if (!s.empty() && fwrite(s.data(), 1, s.size(), f) != s.size()) fail("short write on %s%s", prefix.c_str(), suffix);
     };
     long long read_counter = 0, in_gap = 0, last_batch = 0;
-    std::vector<u64> wofs;
     std::string s_gap, s_txt;
-    char line[128];
     for (u64 b0 = 0; b0 < n_reads; b0 += (u64)max_read_num) {
         const u64 n = std::min<u64>((u64)max_read_num, n_reads - b0);
         last_batch = (long long)n;
         const int alignlen = std::max(plan.long_libs[rd.lib[b0 + n - 1]].map_len, 35);   // ALIGNLEN after the batch's last read (:1198-1204)
-        const u64 w0 = rd.wofs[b0];
-        wofs.resize(n);
-        for (u64 t = 0; t < n; t++) wofs[t] = rd.wofs[b0 + t] - w0;
-        const u64* W = rd.words.data() + w0;
-        const u32* Ln = rd.lens.data() + b0;
-        try { eng.map_long_batch(W, rd.wofs[b0 + n] - w0, wofs.data(), Ln, n, alignlen, hit.data()); }
-        catch (const std::exception& ex) { fail("pgb200: long-read scan failed: %s", ex.what()); }
-        rc.chops(n, P, K, Ln, [&](u64 t) { return W + wofs[t]; });
-        pl.set(hit.data(), n, ci, K, prefix);
+        bm.map(b0, n, alignlen, true, "long-read scan");
         s_gap.clear(); s_txt.clear();
         for (u64 t = 0; t < n; t++) {   // recordLongRead, output1read (prlRead2Ctg.c:456-492, 612-625)
             read_counter++;
             if (!pl.footprint[t]) continue;
-            const int len = (int)Ln[t];
-            const u64* w = W + wofs[t];
+            const int len = (int)bm.lens[t];
             in_gap++;
-            rc.tight(w, len);
-            put(s_gap, len); put(s_gap, (int)pl.ctg[t]); put(s_gap, pl.pos[t]);
-            s_gap.append(reinterpret_cast<const char*>(rc.b.data()), (size_t)(len / 4 + 1));
-            if (fill && len > 0) {
-                s_txt.append(line, (size_t)snprintf(line, sizeof line, ">%d\t%d\t%d\t%c\t%d\t%d\n", len, (int)pl.ctg[t], pl.pos[t], pl.orien[t], 18, 0));
-                for (int i = 0; i < len; i++) s_txt.push_back("ACTG"[(w[i >> 5] >> (2 * (i & 31))) & 3]);
-                s_txt.push_back('\n');
-            }
+            put_gap(s_gap, bm.rc, bm.read(t), len, (int)pl.ctg[t], pl.pos[t]);
+            if (fill && len > 0) put_text(s_txt, bm.read(t), len, (int)pl.ctg[t], pl.pos[t], pl.orien[t], 18, 0);
         }
         put_file(f_gap.get(), s_gap, ".longReadInGap");
         if (fill) put_file(f_txt.get(), s_txt, ".RlongReadInGap");
@@ -450,6 +457,123 @@ struct GzOut {
     void close() { if (f) gzclose(f); f = nullptr; }
     ~GzOut() { close(); }
 };
+
+// prlRead2Ctg once its reads are in: the output files, batches of maxReadNum reads (from max_rd_len), recordAlldgn with its mates
+// (getReadIngap, getPEreadOnContig) and output1read_gz, the closing counts and .peGrads.  long_all: the batches through k_map_long.
+void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, const std::string& log, long long max_read_num, const ContigInfo& ci, int K,
+                     int P, int fill, bool long_all, const std::string& prefix, double* ms_record, double* ms_deflate) {
+    GzOut f_gap, f_short, f_on, f_pe;
+    f_gap.open(prefix + ".readInGap.gz", "wb");
+    if (fill) f_short.open(prefix + ".shortreadInGap.gz", "w");
+    f_on.open(prefix + ".readOnContig.gz", "w");
+    if (fill) f_pe.open(prefix + ".PEreadOnContig.gz", "wb");
+    f_on.write("read\tcontig\tpos\n");
+    fputs(log.c_str(), stderr);
+    struct Grad { int ins; long long bound; int rank, cut; };
+    std::vector<Grad> grads;   // a library's boundary is the count of reads up to its last one (readseq1by1.c:1092-1102)
+    for (size_t r = 0; r < rd.lens.size(); r++)
+        if (r + 1 == rd.lens.size() || rd.lib[r + 1] != rd.lib[r]) {
+            const MapLib& L = plan.libs[rd.lib[r]];
+            grads.push_back({L.avg_ins, (long long)r + 1, L.rank, L.pair_num_cut});
+        }
+    const u64 n_reads = rd.lens.size();
+
+    BatchMapper bm(eng, rd, max_read_num, plan.max_rd_len, ci, K, P, prefix);
+    std::vector<u32>& ctg_arr = bm.pl.ctg;
+    std::vector<int>& pos_arr = bm.pl.pos;
+    const std::vector<char>&orien = bm.pl.orien, &footprint = bm.pl.footprint;
+    long long read_counter = 0, map_counter = 0, in_gap = 0;
+    int alignlen = 0, prev_lib = -1;
+    // everything the writer thread touches is declared before its join guard, so it outlives the thread on every way out
+    std::exception_ptr wr_err;
+    std::string s_gap, s_short, s_on, s_pe;
+    std::thread writer;
+    struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } join_writer{writer};
+    auto join = [&] {
+        const double t_join = host_now();
+        if (writer.joinable()) writer.join();
+        *ms_deflate += host_now() - t_join;
+        if (wr_err) std::rethrow_exception(wr_err);
+    };
+    long long last_batch = 0;
+    for (u64 b0 = 0; b0 < n_reads; b0 += (u64)max_read_num) {
+        const u64 n = std::min<u64>((u64)max_read_num, n_reads - b0);
+        last_batch = (long long)n;
+        for (u64 r = b0; r < b0 + n; r++) {   // ALIGNLEN as it stands after the batch's last read (prlRead2Ctg.c:903-926)
+            const MapLib& L = plan.libs[rd.lib[r]];
+            if (rd.lib[r] != prev_lib) { prev_lib = rd.lib[r]; alignlen = L.avg_ins > 1000 ? std::max(L.map_len, 35) : std::max(L.map_len, 32); }
+            if (L.avg_ins > 1000) alignlen = std::max(alignlen, (int)(rd.lens[r] / 2 + 1));
+        }
+        const double t_rec = bm.map(b0, n, alignlen, long_all, "read scan");
+        // recordAlldgn (prlRead2Ctg.c:627-712) into this batch's byte strings
+        join();
+        s_gap.clear(); s_short.clear(); s_on.clear(); s_pe.clear();
+        auto ins_of = [&](u64 t) { return plan.libs[rd.lib[b0 + t]].avg_ins; };
+        auto output1read = [&](u64 t, char o, int dh) {   // output1read_gz
+            const int len = (int)bm.lens[t];
+            in_gap++;
+            put_gap(s_gap, bm.rc, bm.read(t), len, (int)ctg_arr[t], pos_arr[t]);
+            if (fill && ins_of(t) < 2000 && len > 0) put_text(s_short, bm.read(t), len, (int)ctg_arr[t], pos_arr[t], o, ins_of(t), dh);
+        };
+        auto read_in_gap = [&](u64 t, bool read_one) {   // getReadIngap
+            const u64 r1 = read_one ? t : t - 1, r2 = read_one ? t + 1 : t;
+            const u64 placed = read_one ? r2 : r1, gap = read_one ? r1 : r2;
+            const char o = orien[placed] == '+' ? '-' : '+';
+            ctg_arr[gap] = ctg_arr[placed];
+            pos_arr[gap] = pos_arr[placed] + ins_of(gap) - (int)bm.lens[gap];
+            output1read(gap, o, read_one ? 1 : 2);
+        };
+        auto pe_on_contig = [&](u64 t) {   // getPEreadOnContig
+            if (!(ins_of(t) < 2000 && ins_of(t) == ins_of(t - 1))) return;
+            for (u64 r = t - 1; r <= t; r++) {
+                const int len = (int)bm.lens[r];
+                put(s_pe, len); put(s_pe, (int)ctg_arr[r]); put(s_pe, pos_arr[r]); put(s_pe, orien[r]); put(s_pe, ins_of(r));
+                bm.rc.append_tight(s_pe, bm.read(r), len);
+            }
+        };
+        char line[96];
+        for (u64 t = 0; t < n; t++) {
+            read_counter++;
+            bool rd1gap = false, rd2gap = false;
+            const int ctg_id = (int)ctg_arr[t];
+            if (t % 2 == 1) {
+                if (ctg_arr[t] < 1 && ctg_arr[t - 1] > 0) { read_in_gap(t, false); rd2gap = true; }
+                else if (ctg_arr[t] > 0 && ctg_arr[t - 1] < 1) { read_in_gap(t - 1, true); rd1gap = true; }
+                else if (ctg_arr[t] > 0 && ctg_arr[t - 1] > 0 && fill) pe_on_contig(t);
+            }
+            if (ctg_id < 1) continue;
+            map_counter++;
+            s_on.append(line, (size_t)snprintf(line, sizeof line, "%lld\t%u\t%d\t%c\n", read_counter, ctg_arr[t], pos_arr[t], orien[t]));
+            if (t % 2 == 0) continue;
+            if (footprint[t - 1] && !rd1gap) output1read(t - 1, orien[t] == '+' ? '-' : '+', 1);
+            if (footprint[t] && !rd2gap) output1read(t, orien[t - 1] == '+' ? '-' : '+', 2);
+        }
+        *ms_record += host_now() - t_rec;
+        // the deflate runs beside the next batch's GPU work; its bytes must equal the reference's gz stream, so it is one thread
+        writer = std::thread([&] {
+            try { f_gap.write(s_gap); if (fill) f_short.write(s_short); f_on.write(s_on); if (fill) f_pe.write(s_pe); }
+            catch (...) { wr_err = std::current_exception(); }
+        });
+    }
+    join();
+    if (n_reads && last_batch != max_read_num) {   // a batch that ends exactly at the last read is recorded inside the reference's loop
+        fprintf(stderr, "\nTotal reads         %lld\n", read_counter);
+        fprintf(stderr, "Reads in gaps       %lld\n", in_gap);
+        fprintf(stderr, "Ratio               %.1f%%\n", (float)in_gap / read_counter * 100);
+    }
+    fprintf(stderr, "Reads on contigs    %lld\n", map_counter);
+    fprintf(stderr, "Ratio               %.1f%%\n", (float)map_counter / read_counter * 100);
+    f_on.close();
+    {
+        FILE* fo = ckopen(prefix + ".peGrads", "w");
+        fprintf(fo, "grads&num: %d\t%lld\t%d\n", (int)grads.size(), (long long)n_reads, plan.max_len4all);
+        if (!grads.empty()) fprintf(stderr, "%d pe insert size, the largest boundary is %lld.\n\n", (int)grads.size(), grads.back().bound);
+        else fprintf(stderr, "No paired reads found.\n");
+        for (const Grad& g : grads) fprintf(fo, "%d\t%lld\t%d\t%d\n", g.ins, g.bound, g.rank, g.cut);
+        fclose(fo);
+    }
+    f_gap.close(); f_short.close(); f_pe.close();
+}
 
 int map_stage(int argc, char** argv, int flavour127) {
     const double t_all = host_now();
@@ -494,12 +618,8 @@ int map_stage(int argc, char** argv, int flavour127) {
     const MapPlan plan = map_plan(cfg.c_str());
     if (plan.max_rd_len - K + 1 <= 0) fail("pgb200: max_rd_len %d is shorter than K %d", plan.max_rd_len, K);
     const bool long_pass = plan.long_len >= 1;   // prlRead2Ctg.c:1099-1104
-    // the short reads' stride holds max_rd_len bases, and one more where the long pass raises a cutoff past max_rd_len (load_reads)
-    int short_len = plan.max_rd_len;
-    for (const MapLib& L : plan.libs)
-        for (const PlanEntry& e : L.files) short_len = std::max(short_len, std::min(e.cut, plan.max_rd_len + 1));
     std::unique_ptr<IMapEngine> eng;
-    try { eng.reset(make_map_engine(K, device, short_len)); } catch (const std::exception& ex) { fail("pgb200: %s", ex.what()); }
+    try { eng.reset(make_map_engine(K, device)); } catch (const std::exception& ex) { fail("pgb200: %s", ex.what()); }
     const double t_hash = host_now();
     u64 distinct = 0;
     try { eng->hash_contigs(ctg.packed.data(), ctg.off.back(), ctg.off.data(), ctg.id.data(), ctg.id.size(), &distinct); }
@@ -510,18 +630,17 @@ int map_stage(int argc, char** argv, int flavour127) {
 
     // ---- the reads of both passes, before any output file
     t0 = host_now();
-    const int W64 = eng->words_per_read();
     std::string long_log, short_log;
     // The long pass reads with the fgets reader: long reads are commonly wrapped.  PGB200_MAP_READER=fgets sends the short pass
     // through it as well, a second exact implementation of the reads the parity tests can run over every short-read scenario.  gStr:
     // the long pass allocates it for longReadLen > gLineLen (prlRead2Ctg.c:1133), the short pass for max_rd_len > gLineLen (:826).
     const char* reader_env = getenv("PGB200_MAP_READER");
     const bool fgets_short = reader_env && !strcmp(reader_env, "fgets");
-    const Reads lrd = long_pass ? load_reads(*eng, plan.long_libs, true, plan.long_len, 0, plan.long_len > 5000 ? 1 : 0, &long_log) : Reads{};
+    const Reads lrd = long_pass ? load_reads(*eng, plan.long_libs, true, plan.long_len, plan.long_len > 5000 ? 1 : 0, &long_log) : Reads{};
     MapTimes t_lrd;
     eng->times(&t_lrd);
     const double ms_read_long = host_now() - t0;
-    const Reads rd = load_reads(*eng, plan.libs, false, plan.max_rd_len, W64, fgets_short ? (plan.max_rd_len > 5000 ? 1 : 0) : -1, &short_log);
+    const Reads rd = load_reads(*eng, plan.libs, false, plan.max_rd_len, fgets_short ? (plan.max_rd_len > 5000 ? 1 : 0) : -1, &short_log);
     const double ms_read = host_now() - t0;
     const long long max_read_num = batch_reads("max_rd_len", plan.max_rd_len, K);
     const long long max_long_num = long_pass ? batch_reads("long read length", plan.long_len, K) : 0;
@@ -558,145 +677,8 @@ int map_stage(int argc, char** argv, int flavour127) {
         ci = contig_info(prefix);
         fprintf(stderr, "%d edge(s) in the graph.\n", ci.num_all);
     }
-    GzOut f_gap, f_short, f_on, f_pe;
-    f_gap.open(prefix + ".readInGap.gz", "wb");
-    if (fill) f_short.open(prefix + ".shortreadInGap.gz", "w");
-    f_on.open(prefix + ".readOnContig.gz", "w");
-    if (fill) f_pe.open(prefix + ".PEreadOnContig.gz", "wb");
-    f_on.write("read\tcontig\tpos\n");
-    fputs(short_log.c_str(), stderr);
-    struct Grad { int ins; long long bound; int rank, cut; };
-    std::vector<Grad> grads;   // a library's boundary is the count of reads up to its last one (readseq1by1.c:1092-1102)
-    for (size_t r = 0; r < rd.lens.size(); r++)
-        if (r + 1 == rd.lens.size() || rd.lib[r + 1] != rd.lib[r]) {
-            const MapLib& L = plan.libs[rd.lib[r]];
-            grads.push_back({L.avg_ins, (long long)r + 1, L.rank, L.pair_num_cut});
-        }
-    const u64 n_reads = rd.lens.size();
-
-    // ---- batches of maxReadNum reads, parse1read on the GPU, recordAlldgn here
-    std::vector<MapHit> hit((size_t)std::min<long long>(max_read_num, (long long)std::max<u64>(n_reads, 1)));
-    Placement pl(hit.size());
-    std::vector<u32>& ctg_arr = pl.ctg;
-    std::vector<int>& pos_arr = pl.pos;
-    std::vector<char>&orien = pl.orien, &footprint = pl.footprint;
-    std::vector<u64> wofs;
-    RcSeqModel rc{std::vector<unsigned char>((size_t)plan.max_rd_len, 0)};
-    long long read_counter = 0, map_counter = 0, in_gap = 0;
-    int alignlen = 0, prev_lib = -1;
     double ms_record = 0, ms_deflate = 0;
-    // everything the writer thread touches is declared before its join guard, so it outlives the thread on every way out
-    std::exception_ptr wr_err;
-    std::string s_gap, s_short, s_on, s_pe;
-    std::thread writer;
-    struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } join_writer{writer};
-    long long last_batch = 0;
-    for (u64 b0 = 0; b0 < n_reads; b0 += (u64)max_read_num) {
-        const u64 n = std::min<u64>((u64)max_read_num, n_reads - b0);
-        last_batch = (long long)n;
-        for (u64 r = b0; r < b0 + n; r++) {   // ALIGNLEN as it stands after the batch's last read (prlRead2Ctg.c:903-926)
-            const MapLib& L = plan.libs[rd.lib[r]];
-            if (rd.lib[r] != prev_lib) { prev_lib = rd.lib[r]; alignlen = L.avg_ins > 1000 ? std::max(L.map_len, 35) : std::max(L.map_len, 32); }
-            if (L.avg_ins > 1000) alignlen = std::max(alignlen, (int)(rd.lens[r] / 2 + 1));
-        }
-        const u64* W = rd.words.data() + b0 * W64;
-        const u32* Ln = rd.lens.data() + b0;
-        try {
-            if (long_all) {   // PGB200_MAP_LONG=all: the same batch through k_map_long
-                wofs.resize(n);
-                for (u64 t = 0; t < n; t++) wofs[t] = t * W64;
-                eng->map_long_batch(W, n * W64, wofs.data(), Ln, n, alignlen, hit.data());
-            } else eng->map_batch(W, Ln, n, alignlen, hit.data());
-        } catch (const std::exception& ex) { fail("pgb200: read scan failed: %s", ex.what()); }
-        const double t_rec = host_now();
-        rc.chops(n, P, K, Ln, [&](u64 t) { return W + t * W64; });
-        pl.set(hit.data(), n, ci, K, prefix);
-        // recordAlldgn (prlRead2Ctg.c:627-712) into this batch's byte strings
-        const double t_join = host_now();
-        if (writer.joinable()) writer.join();
-        ms_deflate += host_now() - t_join;
-        if (wr_err) std::rethrow_exception(wr_err);
-        s_gap.clear(); s_short.clear(); s_on.clear(); s_pe.clear();
-        auto ins_of = [&](u64 t) { return plan.libs[rd.lib[b0 + t]].avg_ins; };
-        auto output1read = [&](u64 t, char o, int dh) {   // output1read_gz
-            const int len = (int)Ln[t];
-            in_gap++;
-            rc.tight(W + t * W64, len);
-            put(s_gap, len); put(s_gap, (int)ctg_arr[t]); put(s_gap, pos_arr[t]);
-            s_gap.append(reinterpret_cast<const char*>(rc.b.data()), (size_t)(len / 4 + 1));
-            if (fill && ins_of(t) < 2000 && len > 0) {
-                char line[128];
-                snprintf(line, sizeof line, ">%d\t%d\t%d\t%c\t%d\t%d\n", len, (int)ctg_arr[t], pos_arr[t], o, ins_of(t), dh);
-                s_short += line;
-                const u64* w = W + t * W64;
-                for (int i = 0; i < len; i++) s_short.push_back("ACTG"[(w[i >> 5] >> (2 * (i & 31))) & 3]);
-                s_short.push_back('\n');
-            }
-        };
-        auto read_in_gap = [&](u64 t, bool read_one) {   // getReadIngap
-            const u64 r1 = read_one ? t : t - 1, r2 = read_one ? t + 1 : t;
-            const u64 placed = read_one ? r2 : r1, gap = read_one ? r1 : r2;
-            const char o = orien[placed] == '+' ? '-' : '+';
-            ctg_arr[gap] = ctg_arr[placed];
-            pos_arr[gap] = pos_arr[placed] + ins_of(gap) - (int)Ln[gap];
-            output1read(gap, o, read_one ? 1 : 2);
-        };
-        auto pe_on_contig = [&](u64 t) {   // getPEreadOnContig
-            if (!(ins_of(t) < 2000 && ins_of(t) == ins_of(t - 1))) return;
-            for (u64 r = t - 1; r <= t; r++) {
-                const int len = (int)Ln[r];
-                put(s_pe, len); put(s_pe, (int)ctg_arr[r]); put(s_pe, pos_arr[r]); put(s_pe, orien[r]); put(s_pe, ins_of(r));
-                rc.tight(W + r * W64, len);
-                s_pe.append(reinterpret_cast<const char*>(rc.b.data()), (size_t)(len / 4 + 1));
-            }
-        };
-        char line[96];
-        for (u64 t = 0; t < n; t++) {
-            read_counter++;
-            bool rd1gap = false, rd2gap = false;
-            const int ctg_id = (int)ctg_arr[t];
-            if (t % 2 == 1) {
-                if (ctg_arr[t] < 1 && ctg_arr[t - 1] > 0) { read_in_gap(t, false); rd2gap = true; }
-                else if (ctg_arr[t] > 0 && ctg_arr[t - 1] < 1) { read_in_gap(t - 1, true); rd1gap = true; }
-                else if (ctg_arr[t] > 0 && ctg_arr[t - 1] > 0 && fill) pe_on_contig(t);
-            }
-            if (ctg_id < 1) continue;
-            map_counter++;
-            s_on.append(line, (size_t)snprintf(line, sizeof line, "%lld\t%u\t%d\t%c\n", read_counter, ctg_arr[t], pos_arr[t], orien[t]));
-            if (t % 2 == 0) continue;
-            if (footprint[t - 1] && !rd1gap) output1read(t - 1, orien[t] == '+' ? '-' : '+', 1);
-            if (footprint[t] && !rd2gap) output1read(t, orien[t - 1] == '+' ? '-' : '+', 2);
-        }
-        ms_record += host_now() - t_rec;
-        // the deflate runs beside the next batch's GPU work; its bytes must equal the reference's gz stream, so it is one thread
-        writer = std::thread([&] {
-            try { f_gap.write(s_gap); if (fill) f_short.write(s_short); f_on.write(s_on); if (fill) f_pe.write(s_pe); }
-            catch (...) { wr_err = std::current_exception(); }
-        });
-    }
-    {
-        const double t_join = host_now();
-        if (writer.joinable()) writer.join();
-        ms_deflate += host_now() - t_join;
-        if (wr_err) std::rethrow_exception(wr_err);
-    }
-    if (n_reads && last_batch != max_read_num) {   // a batch that ends exactly at the last read is recorded inside the reference's loop
-        fprintf(stderr, "\nTotal reads         %lld\n", read_counter);
-        fprintf(stderr, "Reads in gaps       %lld\n", in_gap);
-        fprintf(stderr, "Ratio               %.1f%%\n", (float)in_gap / read_counter * 100);
-    }
-    fprintf(stderr, "Reads on contigs    %lld\n", map_counter);
-    fprintf(stderr, "Ratio               %.1f%%\n", (float)map_counter / read_counter * 100);
-    f_on.close();
-    {
-        FILE* fo = ckopen(prefix + ".peGrads", "w");
-        fprintf(fo, "grads&num: %d\t%lld\t%d\n", (int)grads.size(), (long long)n_reads, plan.max_len4all);
-        if (!grads.empty()) fprintf(stderr, "%d pe insert size, the largest boundary is %lld.\n\n", (int)grads.size(), grads.back().bound);
-        else fprintf(stderr, "No paired reads found.\n");
-        for (const Grad& g : grads) fprintf(fo, "%d\t%lld\t%d\t%d\n", g.ins, g.bound, g.rank, g.cut);
-        fclose(fo);
-    }
-    f_gap.close(); f_short.close(); f_pe.close();
+    map_short_reads(*eng, plan, rd, short_log, max_read_num, ci, K, P, fill, long_all, prefix, &ms_record, &ms_deflate);
     print_libs(plan);
     fprintf(stderr, "Time spent on aligning reads: %ds.\n\n", (int)((host_now() - t0) * 1e-3));
     if (verbose) {
