@@ -168,6 +168,19 @@ int pgb200_edge_text_to_sidecar(const char *text, size_t nbytes, int K, int flav
  * like the stage does).  For pipelines that ran the stage with PGB200_EDGE_SIDECAR=only and want the .edge.gz later / in the background. */
 int pgb200_sidecar_to_edge_gz(const char *prefix);
 
+/* gzip files byte-identical to zlib's gzopen(path, "w") + gzwrite + gzclose (default level 6), deflated on the GPU (csrc/deflate.cu).
+ * PGB200_GZ=host writes with zlib itself; the GPU writer is also left for zlib when the runtime zlib's level-6 bytes differ from
+ * the ones it reproduces (pgb200_gz_gpu_exact).  The stages write their .gz outputs through these.                              */
+typedef struct pgb200_gz pgb200_gz;
+/* gzopen(path, "w"): NULL on error (pgb200_last_error says why). */
+pgb200_gz *pgb200_gz_open(const char *path, int device);
+/* gzwrite(file, buf, n): buf is host memory, or device memory on the writer's device when on_device.  0 on success. */
+int pgb200_gz_write(pgb200_gz *h, const void *buf, size_t n, int on_device);
+/* gzclose(file): writes the last block and the trailer and frees the handle (also after an error).  0 on success. */
+int pgb200_gz_close(pgb200_gz *h);
+/* 1: the GPU writer's bytes equal the runtime zlib's deflateInit2(6, Z_DEFLATED, 31, 8, Z_DEFAULT_STRATEGY) on the probe text. */
+int pgb200_gz_gpu_exact(int device);
+
 /* The drop-in stage entry points. */
 int pgb200_pregraph_main(int argc, char **argv, int flavour127);
 int pgb200_map_main(int argc, char **argv, int flavour127);

@@ -23,6 +23,7 @@ EXPORTS = [
     "pgb200_finish_pass1", "pgb200_reset_pass1", "pgb200_sweeps",
     "pgb200_build_layout", "pgb200_node_count", "pgb200_dump_nodes", "pgb200_sample_table", "pgb200_remove_tips", "pgb200_kmer2edges",
     "pgb200_read2edge", "pgb200_output_vertex", "pgb200_edge_text_to_sidecar", "pgb200_sidecar_to_edge_gz", "pgb200_plan_files", "pgb200_cut_chunk", "pgb200_pregraph_main", "pgb200_map_main", "call_pregraph",
+    "pgb200_gz_open", "pgb200_gz_write", "pgb200_gz_close", "pgb200_gz_gpu_exact",
 ]
 
 
@@ -92,6 +93,11 @@ def load():
     lib.pgb200_cut_chunk.argtypes = [C.c_char_p, C.c_size_t, C.c_int]
     lib.pgb200_pregraph_main.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.c_int]
     lib.pgb200_map_main.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.c_int]
+    lib.pgb200_gz_open.restype = C.c_void_p
+    lib.pgb200_gz_open.argtypes = [C.c_char_p, C.c_int]
+    lib.pgb200_gz_write.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]
+    lib.pgb200_gz_close.argtypes = [C.c_void_p]
+    lib.pgb200_gz_gpu_exact.argtypes = [C.c_int]
     _lib = lib
     return lib
 
@@ -255,3 +261,59 @@ def sidecar_to_edge_gz(prefix: str):
     lib = load()
     if lib.pgb200_sidecar_to_edge_gz(prefix.encode()):
         raise EngineError(lib.pgb200_last_error().decode())
+
+
+class GpuGzWriter:
+    """gzopen(path, "w") + gzwrite + gzclose with the deflate on the GPU: the file is byte-identical to zlib's at its default level.
+    PGB200_GZ=host (read at open) writes with zlib instead.  write() takes bytes-like host data, or an int device address with nbytes
+    and on_device=True.  Any piece sizes give the same file."""
+
+    def __init__(self, path, device=0):
+        self.lib = load()
+        self.h = self.lib.pgb200_gz_open(os.fspath(path).encode(), device)
+        if not self.h:
+            raise EngineError(self.lib.pgb200_last_error().decode())
+
+    def write(self, data, nbytes=None, on_device=False):
+        if isinstance(data, int):
+            ptr, n = C.c_void_p(data), nbytes
+        else:
+            mv = memoryview(data).cast("B")
+            n = mv.nbytes if nbytes is None else nbytes
+            if n == 0:
+                return
+            keep = (C.c_char * mv.nbytes).from_buffer_copy(mv) if mv.readonly else (C.c_char * mv.nbytes).from_buffer(mv)
+            ptr = C.cast(keep, C.c_void_p)
+        if self.lib.pgb200_gz_write(self.h, ptr, n, int(on_device)):
+            raise EngineError(self.lib.pgb200_last_error().decode())
+
+    def close(self):
+        if self.h:
+            h, self.h = self.h, None
+            if self.lib.pgb200_gz_close(h):
+                raise EngineError(self.lib.pgb200_last_error().decode())
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def gz_gpu_exact(device=0) -> bool:
+    """True when the GPU writer's bytes equal this process's zlib's on the probe text (otherwise the writers use zlib)."""
+    r = load().pgb200_gz_gpu_exact(device)
+    if r < 0:
+        raise EngineError(load().pgb200_last_error().decode())
+    return r == 1
+
+
+def gzip_bytes(data, device=0) -> bytes:
+    """The gzip file GpuGzWriter writes for `data`, as bytes (through a temporary file)."""
+    import tempfile
+    with tempfile.TemporaryDirectory(prefix="pgb200_gz_") as d:
+        path = os.path.join(d, "x.gz")
+        with GpuGzWriter(path, device) as w:
+            w.write(data)
+        with open(path, "rb") as f:
+            return f.read()

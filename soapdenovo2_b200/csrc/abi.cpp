@@ -1,6 +1,7 @@
 // abi.cpp -- the extern "C" veneer of include/pregraph_b200.h over IEngine.  Errors never unwind across it: every entry point
 // catches, keeps the message for pgb200_last_error() and returns its failure value.
 #include "stage.h"
+#include "deflate.h"
 #include <cstring>
 #include <memory>
 #include <stdexcept>
@@ -111,3 +112,17 @@ extern "C" int pgb200_edge_text_to_sidecar(const char* text, size_t nbytes, int 
     return guarded(-1, [&] { edge_text_to_sidecar(text, nbytes, K, flavour127, num_ed, path); return 0; });
 }
 extern "C" int pgb200_sidecar_to_edge_gz(const char* prefix) { return guarded(-1, [&] { sidecar_to_edge_gz(prefix); return 0; }); }
+
+// ---- gzip writers (deflate.cu)
+struct pgb200_gz { std::unique_ptr<GzFile> f; };
+extern "C" pgb200_gz* pgb200_gz_open(const char* path, int device) {   // gzopen(path, "w")
+    return guarded((pgb200_gz*)nullptr, [&] { return new pgb200_gz{std::unique_ptr<GzFile>(gz_open(path, device))}; });
+}
+extern "C" int pgb200_gz_write(pgb200_gz* h, const void* buf, size_t n, int on_device) {   // gzwrite
+    return guarded(-1, [&] { h->f->write(buf, n, on_device != 0); return 0; });
+}
+extern "C" int pgb200_gz_close(pgb200_gz* h) {   // gzclose
+    std::unique_ptr<pgb200_gz> own(h);
+    return guarded(-1, [&] { h->f->close(); return 0; });
+}
+extern "C" int pgb200_gz_gpu_exact(int device) { return guarded(-1, [&] { return gz_gpu_matches_zlib(device) ? 1 : 0; }); }

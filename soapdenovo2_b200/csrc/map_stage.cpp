@@ -23,6 +23,7 @@
 // string write in order.  It starts as zeros (ckalloc is calloc).
 #include "stage.h"
 #include "map.h"
+#include "deflate.h"
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -442,31 +443,28 @@ void map_long_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, long 
         fprintf(stderr, "Output %lld out of %lld (%.1f)%% reads in gaps.\n", in_gap, read_counter, (float)in_gap / read_counter * 100);
 }
 
+// The map .gz outputs: gzopen + gzwrite bytes, deflated on the GPU of the stage (deflate.cu; PGB200_GZ=host: zlib)
 struct GzOut {
-    gzFile f = nullptr;
+    std::unique_ptr<GzFile> f;
     std::string name;
-    void open(const std::string& n, const char* mode) { name = n; f = gzopen(n.c_str(), mode); if (!f) fail("Cannot open %s. Now exit to system...", n.c_str()); }
-    void write(const std::string& s) {
-        size_t off = 0;
-        while (off < s.size()) {
-            const size_t n = std::min<size_t>(s.size() - off, 1u << 30);
-            if (gzwrite(f, s.data() + off, (unsigned)n) != (int)n) fail("gzwrite failed on %s", name.c_str());
-            off += n;
-        }
+    void open(const std::string& n, int device) {
+        name = n;
+        try { f.reset(gz_open(n, device)); } catch (const std::exception&) { fail("Cannot open %s. Now exit to system...", n.c_str()); }
     }
-    void close() { if (f) gzclose(f); f = nullptr; }
-    ~GzOut() { close(); }
+    void write(const std::string& s) { f->write(s.data(), s.size(), false); }
+    void close() { if (f) f->close(); f.reset(); }
 };
 
 // prlRead2Ctg once its reads are in: the output files, batches of maxReadNum reads (from max_rd_len), recordAlldgn with its mates
 // (getReadIngap, getPEreadOnContig) and output1read_gz, the closing counts and .peGrads.  long_all: the batches through k_map_long.
 void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, const std::string& log, long long max_read_num, const ContigInfo& ci, int K,
                      int P, int fill, bool long_all, const std::string& prefix, double* ms_record, double* ms_deflate) {
+    const int device = getenv("PGB200_DEVICE") ? atoi(getenv("PGB200_DEVICE")) : 0;   // map_stage's device
     GzOut f_gap, f_short, f_on, f_pe;
-    f_gap.open(prefix + ".readInGap.gz", "wb");
-    if (fill) f_short.open(prefix + ".shortreadInGap.gz", "w");
-    f_on.open(prefix + ".readOnContig.gz", "w");
-    if (fill) f_pe.open(prefix + ".PEreadOnContig.gz", "wb");
+    f_gap.open(prefix + ".readInGap.gz", device);
+    if (fill) f_short.open(prefix + ".shortreadInGap.gz", device);
+    f_on.open(prefix + ".readOnContig.gz", device);
+    if (fill) f_pe.open(prefix + ".PEreadOnContig.gz", device);
     f_on.write("read\tcontig\tpos\n");
     fputs(log.c_str(), stderr);
     struct Grad { int ins; long long bound; int rank, cut; };
@@ -549,7 +547,7 @@ void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, cons
             if (footprint[t] && !rd2gap) output1read(t, orien[t - 1] == '+' ? '-' : '+', 2);
         }
         *ms_record += host_now() - t_rec;
-        // the deflate runs beside the next batch's GPU work; its bytes must equal the reference's gz stream, so it is one thread
+        // the deflate runs beside the next batch's GPU work, on the writers' own streams
         writer = std::thread([&] {
             try { f_gap.write(s_gap); if (fill) f_short.write(s_short); f_on.write(s_on); if (fill) f_pe.write(s_pe); }
             catch (...) { wr_err = std::current_exception(); }

@@ -4,11 +4,13 @@
 //   openNextFile / nextValidIndex  prlHashReads.c:903-951, readseq1by1.c:595-674 (library + file-type iteration order)
 //   file writers                   prlHashReads.c:1104-1132 (.kmerFreq), node2edge.c:61-70 (.edge.gz via zlib)
 #include "stage.h"
+#include "deflate.h"
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <stdexcept>
 #include <zlib.h>
 
@@ -176,17 +178,12 @@ void write_kmer_freq(const std::string& prefix, const long long hist[256]) {   /
     for (int i = 1; i < 256; i++) { snprintf(b, sizeof b, "%lld\n", hist[i]); s += b; }
     write_file(prefix + ".kmerFreq", s.data(), s.size());
 }
-// gzopen(name,"w") + gzwrite: same zlib, same default level => the same byte stream as the reference's gzprintf calls
-static void write_edge_gz(const std::string& name, const std::string& text) {
-    gzFile gz = gzopen(name.c_str(), "w");
-    if (!gz) fail("Cannot open %s", name.c_str());
-    size_t off = 0;
-    while (off < text.size()) {
-        size_t n = std::min<size_t>(text.size() - off, 1u << 30);
-        if (gzwrite(gz, text.data() + off, (unsigned)n) != (int)n) { gzclose(gz); fail("gzwrite failed on %s", name.c_str()); }
-        off += n;
-    }
-    gzclose(gz);
+// gzopen(name,"w") + gzwrite: the reference's gzprintf calls write the same byte stream.  The deflate runs on the GPU (deflate.cu;
+// PGB200_GZ=host: zlib), with the same bytes.
+static void write_edge_gz(const std::string& name, const std::string& text, int device) {
+    std::unique_ptr<GzFile> gz(gz_open(name, device));
+    gz->write(text.data(), text.size(), false);
+    gz->close();
 }
 // PGB200_EDGE_SIDECAR unset: <prefix>.edge.gz only (the reference's output).  Set: the sidecar first (a fraction of a second, so a
 // contig that links contig_sidecar.c never waits for the deflate), then the .edge.gz.  "only": the sidecar alone -- the deflate of
@@ -195,7 +192,7 @@ static void write_edge_gz(const std::string& name, const std::string& text) {
 void write_edge_outputs(const std::string& prefix, const std::string& text, const PgParams& p, uint64_t num_ed) {
     const char* sc = getenv("PGB200_EDGE_SIDECAR");
     if (sc) edge_text_to_sidecar(text.data(), text.size(), p.K, p.flavour127, num_ed, prefix + ".edge.b200");
-    if (!(sc && !strcmp(sc, "only"))) write_edge_gz(prefix + ".edge.gz", text);
+    if (!(sc && !strcmp(sc, "only"))) write_edge_gz(prefix + ".edge.gz", text, p.device);
 }
 
 // f2: the edges as a binary sidecar for a `contig` that links csrc/contig_sidecar.c (format: pgb200_edge_sidecar_header).  Converts
@@ -310,6 +307,6 @@ void sidecar_to_edge_gz(const std::string& prefix) {
         if (rec[0] % 100 != 0) text.push_back('\n');
         off += (size_t)rec[3];
     }
-    write_edge_gz(prefix + ".edge.gz", text);
+    write_edge_gz(prefix + ".edge.gz", text, getenv("PGB200_DEVICE") ? atoi(getenv("PGB200_DEVICE")) : 0);
 }
 }   // namespace pgb
