@@ -83,6 +83,9 @@ def main():
         print(f"{r['ms_per_step']:9.2f} {r['launches_per_step']:9.1f}  {r['kernel'][:110]}")
     for i, s in enumerate(spans):
         print(f"step {i}: front end {s['front_end_ms']:.2f} ms (first GPU activity -> start of k_skm_apply), apply {s['apply_ms']:.2f} ms")
+        if s["clear"]:
+            c = s["clear"]
+            print(f"    table clear: +{c['start_ms']:.2f} .. +{c['end_ms']:.2f} ms of the step, ends {c['before_apply_ms']:.2f} ms before k_skm_apply starts")
         for st in s["streams"]:
             print(f"    stream {st['stream']:>3} ({st['role']:>9}): busy {st['busy_ms']:7.2f} ms, idle between its activities {st['gap_ms']:7.2f} ms, "
                   f"first activity at +{st['first_ms']:.2f} ms")
@@ -135,8 +138,10 @@ def step_spans(trace):
             iv = [(e["ts"], min(e["ts"] + e["dur"], t_apply)) for e in es]
             busy = _union_ms(iv)
             names = " ".join(e["name"] for e in es)
-            role = ("partition" if "k_skm_count" in names else "decode" if "k_decode_fast" in names
-                    else "clear" if any(e["cat"] == "gpu_memset" and e["dur"] > 1000 for e in es) else "other")
+            # (a build that splits the partition over two streams shows its count side and its scatter side apart)
+            role = ("partition" if "k_skm_count" in names and "k_skm_scatter" in names else "scatter" if "k_skm_scatter" in names
+                    else "count" if "k_skm_count" in names else "decode" if "k_decode_fast" in names
+                    else "clear" if "k_table_clear" in names or any(e["cat"] == "gpu_memset" and e["dur"] > 1000 for e in es) else "other")
             per_k = {}
             for e in es:
                 per_k[e["name"]] = per_k.get(e["name"], 0.0) + min(e["dur"], t_apply - e["ts"]) / 1e3
@@ -144,7 +149,13 @@ def step_spans(trace):
                          "gap_ms": (max(e for _, e in iv) - iv[0][0]) / 1e3 - busy,
                          "kernels": sorted(per_k.items(), key=lambda kv: -kv[1])})
         rows.sort(key=lambda r: -r["busy_ms"])
-        out.append({"front_end_ms": (t_apply - t0) / 1e3, "apply_ms": apply[0]["dur"] / 1e3, "streams": rows})
+        # the table clear (kernel or memset): its interval relative to the step's first GPU activity, and how long before k_skm_apply it ended
+        clear = [e for e in acts if e["ts"] < t_apply and ("k_table_clear" in e["name"] or (e["cat"] == "gpu_memset" and e["dur"] > 1000))]
+        clr = None
+        if clear:
+            c1 = max(e["ts"] + e["dur"] for e in clear)
+            clr = {"start_ms": (clear[0]["ts"] - t0) / 1e3, "end_ms": (c1 - t0) / 1e3, "before_apply_ms": (t_apply - c1) / 1e3}
+        out.append({"front_end_ms": (t_apply - t0) / 1e3, "apply_ms": apply[0]["dur"] / 1e3, "clear": clr, "streams": rows})
     return out
 
 

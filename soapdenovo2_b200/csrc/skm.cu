@@ -310,14 +310,20 @@ struct SmemTable {
 // One aggregated k-mer -> the global table.  A k-mer lives in exactly one bucket and a bucket is aggregated by one CTA at a time, so
 // when this call CLAIMS the slot nobody else can be touching its {payload, aux} words: they are written with one plain 16-byte store
 // (probe load -> claim CAS -> store: two dependent memory round trips per new key).  A key that already exists (earlier epoch: the
-// arena was flushed mid-stream) is merged with the same 64-bit CAS + atomicMin protocol every other writer uses.
-template <int NW>
-__device__ __forceinline__ bool table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank) {
+// arena was flushed mid-stream, or a lane of this bucket spilled the key, see below) is merged with the same 64-bit CAS + atomicMin
+// protocol every other writer uses.  on_claim(agg) is applied only to an aggregate that becomes the whole entry: the fused end-of-pass
+// sweeps may only see final entries.
+//   The same key can be in the shared-memory table AND in the global table within one bucket: lane A reads an empty slot and then the
+// count at its limit, so it spills the key (SmemTable::find returns 3), while lane B, which read the count a moment earlier, claims that
+// very slot for the same key.  A few keys per pass at 30x.  Their instances are split over the two copies; the flush merges the
+// shared-memory part UNSWEPT into the entry the spill made, and that entry is on the launch's spill list, which is swept afterwards.
+template <int NW, class OnClaim>
+__device__ __forceinline__ bool table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank, OnClaim on_claim) {
     bool claimed;
     u64 idx = table_find_or_claim(t, k, &claimed);
     Slot<NW>* s = t.slots + idx;
     if (claimed) {
-        stcg128(&s->payload, U128{agg, rank});
+        stcg128(&s->payload, U128{on_claim(agg), rank});
         return true;
     }
     u64 cur = ldcg64(&s->payload);
@@ -796,11 +802,10 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             Kmer<NW> k;
 #pragma unroll
             for (int w = 0; w < NW; w++) k.w[w] = st.key[w * SKM_SLOTS + idx];
-            u64 agg = st.pay[idx];
-            if (a.sweep) agg = sweep_payload(agg, a.D, sw_rem, sw_lin, s_sw.hist);   // this launch is the whole pass: the entry is final
-            const bool fresh = table_merge(tab, k, agg, st.rnk[idx]);
-            my_new += fresh;
-            if (a.sweep && !fresh) atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], (unsigned long long)a.spill_cap + 1ull);   // (cannot happen in an empty table: makes the host run k_sweep)
+            // this launch is the whole pass (a.sweep): an entry this flush creates is final and is swept here; one that a spill of this
+            // bucket created already is on the spill list and is swept from there
+            my_new += table_merge(tab, k, st.pay[idx], st.rnk[idx],
+                                  [&](u64 agg) { return a.sweep ? sweep_payload(agg, a.D, sw_rem, sw_lin, s_sw.hist) : agg; });
             st.key[idx] = EMPTY64;
             st.pay[idx] = PAYLOAD_FRESH;
             st.rnk[idx] = ~0ull;
