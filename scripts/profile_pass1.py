@@ -1,7 +1,8 @@
 """Where the time of one pass 1 goes: the bench workload (bench.py's own generator and budget, configs[1] shape by default) fed from
 HBM, warm-up steps, then timed steps under torch.profiler with CUDA activities.  Writes DIR/kernels.json (per-kernel GPU time per
 step and launches per step, largest first, with the GPU's name and power limit) and DIR/trace.json (Chrome trace), and prints the
-table.  Per timed step it also prints the front-end span (first GPU activity of the step -> start of k_skm_apply) and, inside that
+table.  Per timed step it also prints the front-end span (first GPU activity of the step -> start of k_skm_apply), the time of the
+region build behind it (k_table_build + k_merge_remnants, which the engine books with the aggregation) and, inside the front-end
 span, every stream's busy time and the idle time between its activities.  The per-kernel sums add up durations of kernels that share
 the SMs; run once more with CUDA_LAUNCH_BLOCKING=1 for each kernel's time with nothing beside it.  PGB200_BUILD selects a variant
 build as everywhere else.
@@ -82,7 +83,8 @@ def main():
     for r in rows[:25]:
         print(f"{r['ms_per_step']:9.2f} {r['launches_per_step']:9.1f}  {r['kernel'][:110]}")
     for i, s in enumerate(spans):
-        print(f"step {i}: front end {s['front_end_ms']:.2f} ms (first GPU activity -> start of k_skm_apply), apply {s['apply_ms']:.2f} ms")
+        print(f"step {i}: front end {s['front_end_ms']:.2f} ms (first GPU activity -> start of k_skm_apply), apply {s['apply_ms']:.2f} ms, "
+              f"region build {s['build_ms']:.2f} ms (k_table_build + k_merge_remnants)")
         if s["clear"]:
             c = s["clear"]
             print(f"    table clear: +{c['start_ms']:.2f} .. +{c['end_ms']:.2f} ms of the step, ends {c['before_apply_ms']:.2f} ms before k_skm_apply starts")
@@ -155,7 +157,8 @@ def step_spans(trace):
         if clear:
             c1 = max(e["ts"] + e["dur"] for e in clear)
             clr = {"start_ms": (clear[0]["ts"] - t0) / 1e3, "end_ms": (c1 - t0) / 1e3, "before_apply_ms": (t_apply - c1) / 1e3}
-        out.append({"front_end_ms": (t_apply - t0) / 1e3, "apply_ms": apply[0]["dur"] / 1e3, "clear": clr, "streams": rows})
+        build = sum(e["dur"] for e in acts if "k_table_build" in e["name"] or "k_merge_remnants" in e["name"]) / 1e3
+        out.append({"front_end_ms": (t_apply - t0) / 1e3, "apply_ms": apply[0]["dur"] / 1e3, "build_ms": build, "clear": clr, "streams": rows})
     return out
 
 

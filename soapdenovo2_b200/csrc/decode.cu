@@ -382,6 +382,7 @@ void EngineT<NW>::feed_text(const char* text, size_t nbytes, bool on_device, int
     // updates).  PGB200_SKM=0|1 forces one of them.
     const bool use_skm = prm_.world > 1 || skm_mode_ > 0 || (skm_mode_ < 0 && on_device);
     cudaStream_t sd = use_skm ? st_dec_ : st_;   // the per-instance insert needs exact counters per chunk: one stream
+    if (!use_skm) clear_table_if_dirty();        // the inserts need an empty table: its clear runs beside this chunk's decode
     const unsigned char* d_text = nullptr;
     const bool host_src = !on_device;
     if (host_src) {

@@ -72,9 +72,10 @@ struct ReadChunk {
 };
 
 enum Counter { C_DISTINCT = 0, C_INSTANCES, C_KEPT, C_LINEAR, C_REMOVED, C_MISC0, C_MISC1, C_MISC2, C_BADFMT, C_XERR, C_XUSED, C_RESERVED, C_DEFER, C_MAXU,
-               C_XSEGS, C_XEPOCH, C_SPILLKEYS, C_REDO, C_SKM_STAGED, C_SKM_DRAINED, C_COUNT };
-               // C_SPILLKEYS: keys the aggregation stored WITHOUT the fused sweeps; C_REDO: records decoded by the general rules (k_decode_fix);
-               // C_SKM_STAGED / C_SKM_DRAINED: records an aggregation read, distinct records it expanded (k_skm_apply)
+               C_XSEGS, C_XEPOCH, C_SPILLKEYS, C_REDO, C_SKM_STAGED, C_SKM_DRAINED, C_CARRY, C_BIN_OVF, C_COUNT };
+               // C_SPILLKEYS: keys a region build stored WITHOUT the fused sweeps (its carries); C_REDO: records decoded by the general rules
+               // (k_decode_fix); C_SKM_STAGED / C_SKM_DRAINED: records an aggregation read, distinct records it expanded (k_skm_apply);
+               // C_CARRY: entries on the region build's remnant list (bin overflow + carries), C_BIN_OVF: the bin overflow among them
 
 // What an aggregation launch reports: C_XERR .. C_MAXU, read with one copy
 struct FlushOutcome { u64 xerr, xused, reserved, defer, maxu; };
@@ -86,14 +87,14 @@ static_assert(C_XUSED == C_XERR + 1 && C_RESERVED == C_XERR + 2 && C_DEFER == C_
 static_assert(C_REMOVED == C_LINEAR + 1, "C_LINEAR, C_REMOVED are reset together");
 static_assert(C_INSTANCES == C_DISTINCT + 1 && C_KEPT == C_DISTINCT + 2, "absorb writes C_DISTINCT .. C_KEPT with one copy");
 
-// Whether the end-of-pass sweeps (K4) already ran inside this pass's aggregation launch.  The launch can apply them to every entry it
-// stores only when it is the pass so far (empty table, no launch and no per-instance insert before it): each entry is then final, and
-// one pass over the table is saved.  Without -d the sweeps only SET flags that k_sweep recomputes, so the launch may do them
-// speculatively; with -d the link counters are zeroed for good, so the launch must be known to be the last of the pass (finish_pass1 on
-// one GPU).  Whatever touches the table afterwards -- another launch, a per-instance insert, a table growth, more unswept keys than the
-// spill list holds -- makes the result Plain.
+// Whether the end-of-pass sweeps (K4) already ran inside this pass's aggregation launch.  They can, when the launch is the pass so far (no
+// key in the table, no launch and no per-instance insert before it): such a launch builds the table region by region (k_table_build,
+// skm.cu), every entry is final when its region is written, and one pass over the table is saved.  Without -d the sweeps only SET flags
+// that k_sweep recomputes, so the build may do them speculatively; with -d the link counters are zeroed for good, so the launch must be
+// known to be the last of the pass (finish_pass1 on one GPU).  Whatever touches the table afterwards -- another launch, a per-instance
+// insert, a table growth, a bin overflow, more carries than the spill list holds -- makes the result Plain.
 //   Untouched  no aggregation launch and no per-instance insert since reset_pass1
-//   Fused      this pass's only launch applied the sweeps and they still hold: sweeps() only sweeps the spill list
+//   Fused      this pass's only launch was a region build that applied the sweeps, and they still hold: sweeps() sweeps the carries only
 //   Plain      anything else: sweeps() runs k_sweep over the whole table
 enum class PassSweeps { Untouched, Fused, Plain };
 
@@ -117,7 +118,8 @@ void decode_records(const unsigned char* d_text, size_t nbytes, const DecodeLine
 // The aggregation launch whose outcome (deferred buckets, time) has not been read yet
 struct PendingFlush {
     bool pending = false;
-    bool sweep = false;   // the launch (and its deferred re-runs) applies the end-of-pass sweeps
+    bool region = false;  // the launch wrote its aggregates to the bins and k_table_build made the table from them
+    bool sweep = false;   // ... and the build applied the end-of-pass sweeps
     int half = 0;         // the arena half it reads
 };
 
@@ -170,9 +172,10 @@ public:
     DevBuf text_bufs_[2], line_buf_, scan_buf_, hist_buf_;
     int text_flip_ = 0;
     Stream st_copy_;            // H2D of chunk i+1 overlaps the insert of chunk i
-    Stream st_clear_;           // the table clear between two passes (reset_pass1)
+    Stream st_clear_;           // the table clear, queued before the first write that needs an empty table (clear_table_if_dirty)
     Event ev_clear_;
     bool clear_pending_ = false;
+    bool table_dirty_ = false;  // the table memory holds no valid table (fresh allocation, or a previous pass): cleared lazily
     Event ev_copy_;
     void settle_timing();                        // waits for every fed chunk's kernels and books their times
     void settle_oldest();
@@ -207,13 +210,20 @@ public:
     u32 xa_seg_idx_ = 0;
     PendingFlush flush_;
     PassSweeps pass_sweeps_ = PassSweeps::Untouched;
-    DevBuf spill_list_;                // slots of the keys a Fused launch stored unswept (instances that did not fit a bucket's shared-memory table)
+    DevBuf spill_list_;                // slots of the keys a Fused launch stored unswept (the region build's carries)
     static constexpr u64 SPILL_CAP = 1ull << 22;
+    // the region build (PGB200_TABLE_BUILD=region, the default; merge: every launch merges into the global table with the CAS protocol)
+    bool table_build_region_ = true;
+    int region_log2_ = 0;              // slots per region (and bin capacity) = 2^region_log2_
+    DevBuf bin_cursor_;                // [regions] u32: entries the aggregation stored in each bin
+    DevBuf carry_buf_;                 // remnant list: entries past their bin's capacity, then the build's carries (Slot<NW> format)
+    u64 carry_cap_ = 0;
+    void table_build_launch();
     Pinned<FlushOutcome> h_outcome_;   // as of the end of the last aggregation launch
     Event ev_flush_begin_, ev_flush_;
     void skm_close_epoch(bool hard);
     void skm_flush_complete();
-    void skm_launch_apply(const u32* list, u32 n_list, u32* deferred_out);
+    void skm_launch_apply(const u32* list, u32 n_list, u32* deferred_out, bool region);
     std::vector<u64> xa_reads_cum_;   // reads fed in this epoch after 0, 1, 2, ... chunks (the fill known to the host lags behind)
     u64 skm_room_estimate(u64 n_rec);
     bool xa_dirty_ = false;
@@ -238,7 +248,9 @@ public:
 
     // helpers
     void ensure_table_bound(u64 have, u64 incoming);
-    void create_table_if_needed();
+    void create_table_if_needed(bool clean = true);   // clean = false: the caller overwrites every slot (region build)
+    void clear_table_if_dirty();
+    void alloc_first_table();
     std::vector<DevBuf> arena_;   // read-store blocks
     size_t arena_used_ = 0;
     void* arena_alloc(size_t bytes);
@@ -250,8 +262,8 @@ public:
         PG_CUDA(cudaStreamSynchronize(st_));
         if (clear_pending_) { PG_CUDA(cudaStreamSynchronize(st_clear_)); clear_pending_ = false; }
     }
-    // reset_pass1 clears the table on its own stream: the next pass's decode and partition kernels (which do not touch the table) run
-    // beside the 17 GB memset instead of behind it.  Whoever touches the table next orders the insert stream behind the clear.
+    // The table clear runs on its own stream: decode and partition kernels (which do not touch the table) run beside the 17 GB memset
+    // instead of behind it.  Whoever touches the table next orders the insert stream behind the clear.
     void join_table_clear() {
         if (!clear_pending_) return;
         PG_CUDA(cudaStreamWaitEvent(st_, ev_clear_, 0));

@@ -107,10 +107,21 @@ __global__ void k_rehash(Table<NW> oldt, Table<NW> newt) {
 template <int NW>
 void EngineT<NW>::alloc_table(u64 cap) {
     tab_buf_.alloc(cap * sizeof(Slot<NW>));
-    PG_CUDA(cudaMemsetAsync(tab_buf_.p, 0xFF, cap * sizeof(Slot<NW>), st_));
+    table_dirty_ = true;   // cleared by the first write that needs an empty table (a region build writes every slot itself)
     tab_.slots = tab_buf_.template as<Slot<NW>>();
     tab_.mask = cap - 1;
     cap_ = cap;
+}
+
+// Queue the clear of a table that holds no valid table (a fresh allocation or a previous pass's table).  It runs on its own stream;
+// create_table_if_needed orders the insert stream behind it.
+template <int NW>
+void EngineT<NW>::clear_table_if_dirty() {
+    if (!table_dirty_ || !tab_.slots) return;
+    PG_CUDA(cudaMemsetAsync(tab_buf_.p, 0xFF, cap_ * sizeof(Slot<NW>), st_clear_));
+    PG_CUDA(cudaEventRecord(ev_clear_, st_clear_));
+    clear_pending_ = true;
+    table_dirty_ = false;
 }
 
 template <int NW>
@@ -144,9 +155,14 @@ bool EngineT<NW>::grow_table_for(u64 need, double load, u64 headroom, bool parti
 }
 
 template <int NW>
-void EngineT<NW>::create_table_if_needed() {
+void EngineT<NW>::create_table_if_needed(bool clean) {
+    if (!tab_.slots) alloc_first_table();
+    if (clean) clear_table_if_dirty();
     join_table_clear();
-    if (tab_.slots) return;
+}
+
+template <int NW>
+void EngineT<NW>::alloc_first_table() {
     u64 want = prm_.table_slots;
     if (want) {
         alloc_table(next_pow2(want < 1024 ? 1024 : want));
@@ -217,6 +233,7 @@ void EngineT<NW>::finish_pass1(Pass1Stats* st) {
     settle_timing();
     sync();
     skm_flush_complete();
+    create_table_if_needed();   // a pass that stored nothing leaves the previous pass's table: the later phases read an empty one
     read_counters();
     if (pass_sweeps_ == PassSweeps::Fused && h_cnt_[C_SPILLKEYS] > SPILL_CAP) pass_sweeps_ = PassSweeps::Plain;   // more unswept keys than the list holds
     check_format_counter();
@@ -295,13 +312,9 @@ void EngineT<NW>::reset_pass1() {
     order_buf_.release();
     n_nodes_ = 0;
     sync();
-    // the table is cleared on its own stream WITHOUT waiting: the next pass starts with decoding and partitioning, which do not touch
-    // the table; whatever touches it next joins the clear first (create_table_if_needed -> join_table_clear)
-    if (tab_.slots) {
-        PG_CUDA(cudaMemsetAsync(tab_buf_.p, 0xFF, cap_ * sizeof(Slot<NW>), st_clear_));
-        PG_CUDA(cudaEventRecord(ev_clear_, st_clear_));
-        clear_pending_ = true;
-    }
+    // no clear here: the pass's first aggregation launch builds the table region by region and writes every slot, so only a first
+    // write that needs an empty table queues the clear (create_table_if_needed -> clear_table_if_dirty)
+    table_dirty_ = tab_.slots != nullptr;
     for (int i = 0; i < C_COUNT; i++) h_cnt_[i] = 0;
     if (prm_.verbose >= 2) fprintf(stderr, "[pgb200] reset_pass1: %.2f ms host\n", host_now() - t0);
 }
@@ -434,6 +447,10 @@ EngineT<NW>::EngineT(const PgParams& p) : prm_(p) {
     PG_CUDA(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, p.device));
     if (const char* g = getenv("PGB200_SKM")) skm_mode_ = atoi(g) ? 1 : 0;
     if (const char* g = getenv("PGB200_SKM_FLUSH_EVERY")) skm_flush_every_ = atoi(g);
+    if (const char* g = getenv("PGB200_TABLE_BUILD")) {
+        if (!strcmp(g, "merge")) table_build_region_ = false;
+        else if (strcmp(g, "region")) throw std::runtime_error("pgb200: PGB200_TABLE_BUILD must be region or merge");
+    }
     if (p.world > 1) skm_mode_ = 1;   // records are the only exchange format
     kp_ = make_kparams<NW>(p.K);
     for (Stream* s : {&st_, &st_copy_, &st_clear_, &st_dec_}) PG_CUDA(cudaStreamCreateWithFlags(&s->h, cudaStreamNonBlocking));

@@ -11,10 +11,12 @@
 //                                     for the others.  Partition and "all-to-all" are the same kernel; no library collective, no
 //                                     staging buffer, no second pass over the records.
 //   flush (end of pass 1 / arena full):  k_skm_apply over the owned buckets; buckets whose worst case does not fit the global table
-//                                     are deferred, the table grows, the deferred buckets run again.  When the launch is the whole
-//                                     pass (the normal case) the end-of-pass sweeps -- delow, linear flag, coverage histogram
-//                                     (thread_delow / thread_mark / freqStat, prlHashReads.c:953-1132) -- are applied to every
-//                                     entry as it is stored: no separate pass over the table.
+//                                     are deferred, the table grows, the deferred buckets run again.  When the table holds no key yet
+//                                     (the pass's first launch: the normal case is one launch per pass) the launch stores its
+//                                     aggregates into bins -- the table memory of their home region, no probe, no claim -- and
+//                                     k_table_build makes each region in shared memory and writes it whole: no table clear, and the
+//                                     end-of-pass sweeps -- delow, linear flag, coverage histogram (thread_delow / thread_mark /
+//                                     freqStat, prlHashReads.c:953-1132) -- are applied to every entry as its region is written.
 // Replaces, for the same result, chopKmer4read + the owner filter + put_kmerset (prlHashReads.c:163-259, 79-90; newhash.c:473-528).
 #include "engine_impl.cuh"
 #include "skm.cuh"
@@ -307,26 +309,9 @@ struct SmemTable {
     }
 };
 
-// One aggregated k-mer -> the global table.  A k-mer lives in exactly one bucket and a bucket is aggregated by one CTA at a time, so
-// when this call CLAIMS the slot nobody else can be touching its {payload, aux} words: they are written with one plain 16-byte store
-// (probe load -> claim CAS -> store: two dependent memory round trips per new key).  A key that already exists (earlier epoch: the
-// arena was flushed mid-stream, or a lane of this bucket spilled the key, see below) is merged with the same 64-bit CAS + atomicMin
-// protocol every other writer uses.  on_claim(agg) is applied only to an aggregate that becomes the whole entry: the fused end-of-pass
-// sweeps may only see final entries.
-//   The same key can be in the shared-memory table AND in the global table within one bucket: lane A reads an empty slot and then the
-// count at its limit, so it spills the key (SmemTable::find returns 3), while lane B, which read the count a moment earlier, claims that
-// very slot for the same key.  A few keys per pass at 30x.  Their instances are split over the two copies; the flush merges the
-// shared-memory part UNSWEPT into the entry the spill made, and that entry is on the launch's spill list, which is swept afterwards.
-template <int NW, class OnClaim>
-__device__ __forceinline__ bool table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank, OnClaim on_claim) {
-    bool claimed;
-    u64 idx = table_find_or_claim(t, k, &claimed);
-    Slot<NW>* s = t.slots + idx;
-    if (claimed) {
-        stcg128(&s->payload, U128{on_claim(agg), rank});
-        return true;
-    }
-    u64 cur = ldcg64(&s->payload);
+// A partial aggregate into an entry whose payload word was `cur` when read: the 64-bit CAS + atomicMin protocol every writer uses
+template <int NW>
+__device__ __forceinline__ void slot_merge(Slot<NW>* s, u64 cur, u64 agg, u64 rank) {
     for (;;) {
         u64 nxt = payload_merge(cur, agg);
         if (nxt == cur) break;
@@ -335,7 +320,62 @@ __device__ __forceinline__ bool table_merge(const Table<NW>& t, const Kmer<NW>& 
         cur = old;
     }
     atomicMin(&s->aux, rank);
+}
+
+// One aggregated k-mer -> the global table (merge mode, or a launch after the pass's first).  A k-mer lives in exactly one bucket and a
+// bucket is aggregated by one CTA at a time, so when this call CLAIMS the slot nobody else can be touching its {payload, aux} words:
+// they are written with one plain 16-byte store (probe load -> claim CAS -> store: two dependent memory round trips per new key).  A key
+// that already exists (earlier epoch, or a lane of this bucket spilled the key) is merged with slot_merge.
+template <int NW>
+__device__ __forceinline__ bool table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank) {
+    bool claimed;
+    u64 idx = table_find_or_claim(t, k, &claimed);
+    Slot<NW>* s = t.slots + idx;
+    if (claimed) {
+        stcg128(&s->payload, U128{agg, rank});
+        return true;
+    }
+    slot_merge(s, ldcg64(&s->payload), agg, rank);
     return false;
+}
+
+// One whole slot {key, payload, rank} with 16-byte stores (fire and forget)
+template <int NW>
+__device__ __forceinline__ void slot_store(Slot<NW>* s, const Kmer<NW>& k, u64 pay, u64 rank) {
+    u64* d = reinterpret_cast<u64*>(s);
+    if (NW == 2) {
+        st256(d, k.w[0], k.w[1], pay, rank);
+    } else {
+        stcg128(d, U128{k.w[0], k.w[1]});
+        stcg128(d + 2, U128{k.w[2], k.w[3]});
+        stcg128(d + 4, U128{pay, rank});
+    }
+}
+
+// Region mode: an aggregate of key k goes to its bin, the table memory of its home region (table_hash(k) & mask) >> region_log2, at
+// the position one atomicAdd on the bin's cursor hands out.  Past the bin's capacity (the region's slot count) it goes to the remnant
+// list, which k_merge_remnants merges after the build; past the list's capacity it is counted only, and the host builds the pass again
+// in merge mode (skm_flush_complete).
+struct BinArgs {
+    u32* cursor;      // [regions]
+    void* remnant;    // Slot<NW>[cap]
+    u64 remnant_cap;
+    int region_log2;
+};
+template <int NW>
+__device__ __forceinline__ void bin_store(const Table<NW>& t, const BinArgs& b, u64* counters, const Kmer<NW>& k, u64 pay, u64 rank) {
+    const u64 bin = (table_hash(k) & t.mask) >> b.region_log2;
+    const u32 at = atomicAdd(&b.cursor[bin], 1u);
+    Slot<NW>* s;
+    if (at < (1u << b.region_log2)) {
+        s = t.slots + (bin << b.region_log2) + at;
+    } else {
+        atomicAdd(&counters[C_BIN_OVF], 1ull);
+        const u64 j = atomicAdd(&counters[C_CARRY], 1ull);
+        if (j >= b.remnant_cap) return;
+        s = reinterpret_cast<Slot<NW>*>(b.remnant) + j;
+    }
+    slot_store(s, k, pay, rank);
 }
 
 struct SkmFlushArgs {
@@ -379,11 +419,7 @@ struct SkmApplyArgs {
     u64* counters;            // C_RESERVED: keys the table is committed to hold; C_DEFER / C_MAXU: deferred buckets, their largest bound
     u64 limit;
     u32* deferred;
-    int sweep;                // 1: the flush applies the end-of-pass sweeps to every entry it stores (the launch is the whole pass)
-    int D;
-    u64* hist;                // [256] coverage histogram of the swept entries
-    u64* spill_list;          // slots of the keys stored unswept (spilled instances): the host sweeps them afterwards
-    u64 spill_cap;
+    BinArgs bins;             // k_skm_apply<NW, true>: where the aggregates go
     int collapse;             // SKM_COLLAPSE_OFF / _ON / _AUTO (PGB200_SKM_COLLAPSE): both ways of filling the buffer are exact.  256-bit
                               // keys only: at K <= 63 records repeat (0.553 of them distinct at 30x) and the kernel always collapses;
                               // its register budget at 4 CTAs per SM has no room for the copy path (DESIGN.md §5)
@@ -533,7 +569,8 @@ __device__ __forceinline__ void skm_stage_window(u64* stage, u64* bar, const u64
     }
 }
 
-// One CTA per bucket (static round-robin over the list: buckets are hash-uniform), one shared-memory table per CTA.  A bucket is
+// One CTA per bucket (static round-robin over the list: buckets are hash-uniform), one shared-memory table per CTA.  REGION: the
+// aggregates go to their bins (bin_store) and k_table_build makes the table; else they are merged into the table (table_merge).  A bucket is
 // processed window by window (skm_stage_window); the table persists over the windows and is flushed once per bucket.  When a window
 // has landed, one thread per record collapses it into the buffer of distinct records (skm_dedup_insert): at 30x most records of a
 // bucket are copies of another one.  The buffer is drained into the table when it is full and at the end of the bucket: one thread
@@ -541,7 +578,7 @@ __device__ __forceinline__ void skm_stage_window(u64* stage, u64* bar, const u64
 // instances into contiguous slices and take 32 CONSECUTIVE instances per step -- all lanes busy whatever the run lengths: the
 // records that start inside the step come from one lookahead load of P, and every lane builds its k-mer and reverse complement with
 // two shifts of shared-memory words (skm_instance_staged) and applies it as many times as its record occurred.
-template <int NW>
+template <int NW, bool REGION>
 __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k_skm_apply(Table<NW> tab, KParams<NW> kp, SkmApplyArgs a) {
     constexpr int RW = NW + 2, WARPS = SKM_APPLY_THREADS / 32, C = SKM_BUF_RECS, SKM_W = skm_w<NW>(), SKM_DEDUP_SLOTS = skm_dd_slots<NW>();
     constexpr bool COPY_PATH = NW > 2;   // SKM_COLLAPSE_OFF / _AUTO exist for 256-bit keys only (see SkmApplyArgs::collapse)
@@ -562,7 +599,6 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     __shared__ u64 s_staged, s_drained;   // records staged, distinct records drained (PGB200_SKM_STATS)
     __shared__ u32 s_coll, s_ad_n;        // collapse the next bucket's records; buckets since the auto mode last decided
     __shared__ u64 s_ad_staged, s_ad_drained;   // s_staged, s_drained when it did
-    __shared__ SweepTally s_sw;   // the fused sweeps (a.sweep)
 #ifdef SKM_PHASE_CLOCKS
     __shared__ u64 s_wall[SKM_WALL_PHASES];
     __shared__ long long s_wall_last;
@@ -593,9 +629,6 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         mbar_init(&s_bar[0], 1);
         mbar_init(&s_bar[1], 1);
     }
-    static_assert(SKM_APPLY_THREADS == 256, "one histogram bin per thread");
-    s_sw.clear();
-    unsigned sw_lin = 0, sw_rem = 0;
     const int n_segs = (int)a.segs->n;
     const u32* my_so = tid < n_segs ? a.segs->segoff[tid] : nullptr;
     const u64* my_recs = tid < n_segs ? a.segs->recs[tid] : nullptr;
@@ -721,14 +754,14 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
                         st.apply(slot, in.left, in.right, rank, c);
                         SKM_ACC(3, t_upd);
                     } else if (state == 3) {
-                        // bucket holds more distinct k-mers than the shared-memory table: this k-mer goes to HBM directly (same result;
-                        // the CAS protocol, since lanes may spill the same new key at once)
-                        u64 at;
-                        const bool fresh = table_insert(tab, in.canon, in.left, in.right, rank, &at, c);
-                        if (fresh) atomicAdd(&s_new, 1u);
-                        if (fresh && a.sweep) {   // its other instances follow the same way: swept after the launch, from this list
-                            const u64 sn = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
-                            if (sn < a.spill_cap) a.spill_list[sn] = at;
+                        // bucket holds more distinct k-mers than the shared-memory table: this k-mer goes to HBM directly (same result).
+                        // Region mode: to its bin as a partial aggregate (counted as a new key: the bound the CTA's credit is settled
+                        // with); else the CAS protocol, since lanes may spill the same new key at once.
+                        if constexpr (REGION) {
+                            bin_store(tab, a.bins, a.counters, in.canon, payload_apply_n(PAYLOAD_FRESH, in.left, in.right, c), rank);
+                            atomicAdd(&s_new, 1u);
+                        } else if (table_insert(tab, in.canon, in.left, in.right, rank, nullptr, c)) {
+                            atomicAdd(&s_new, 1u);
                         }
                         SKM_ACC(4, t_upd);
                     }
@@ -802,10 +835,12 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
             Kmer<NW> k;
 #pragma unroll
             for (int w = 0; w < NW; w++) k.w[w] = st.key[w * SKM_SLOTS + idx];
-            // this launch is the whole pass (a.sweep): an entry this flush creates is final and is swept here; one that a spill of this
-            // bucket created already is on the spill list and is swept from there
-            my_new += table_merge(tab, k, st.pay[idx], st.rnk[idx],
-                                  [&](u64 agg) { return a.sweep ? sweep_payload(agg, a.D, sw_rem, sw_lin, s_sw.hist) : agg; });
+            if constexpr (REGION) {
+                bin_store(tab, a.bins, a.counters, k, st.pay[idx], st.rnk[idx]);
+                my_new++;   // an upper bound of the new keys: the CTA's credit is settled with it, C_DISTINCT comes from the build
+            } else {
+                my_new += table_merge(tab, k, st.pay[idx], st.rnk[idx]);
+            }
             st.key[idx] = EMPTY64;
             st.pay[idx] = PAYLOAD_FRESH;
             st.rnk[idx] = ~0ull;
@@ -828,8 +863,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
     }
     __syncthreads();
     if (tid == 0 && credit) atomicAdd((unsigned long long*)&a.counters[C_RESERVED], (unsigned long long)(0ull - credit));
-    s_sw.flush(sw_lin, sw_rem, a.hist, &a.counters[C_LINEAR], &a.counters[C_REMOVED]);   // (all zero without a.sweep)
-    if (tid == 0 && s_tot_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_tot_new);
+    if (!REGION && tid == 0 && s_tot_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_tot_new);
     if (tid == 0 && s_staged) {
         atomicAdd(&a.counters[C_SKM_STAGED], s_staged);
         atomicAdd(&a.counters[C_SKM_DRAINED], s_drained);
@@ -843,6 +877,152 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
         atomicAdd(&g_skm_wall_clk[SKM_WALL_PHASES + 1], 1ull);
     }
 #endif
+}
+
+// ------------------------------------------------------------------------------------------------ region build
+// The table of a launch into an empty table is a pure function of its aggregates, and its slot positions are private to the engine (any
+// valid linear-probing placement will do): so it is built like a partitioned hash build.  One CTA per region (grid-stride): fill the
+// region in shared memory with EMPTY, read the bin's entries (the region's own table memory, written by k_skm_apply<NW, true>), find or
+// claim each key by linear probing WITHOUT wrap-around and merge its partials, sweep every occupied slot, write the region out whole,
+// empty slots included.  Every partial of a key lands in the same bin, and slots never empty again, so a key is either entirely in the
+// region -- final, and swept here -- or all its probes run off the region's end: a carry, appended to the remnant list and merged by
+// k_merge_remnants once every region is written.  Regions of 64 KB let 3 CTAs share an SM (one region's fill, read, probe and
+// write-back overlap another's); a bin holds 2048 (K <= 63) or 1024 slots' worth of entries, twice the expected fill at 0.85 load.
+constexpr int TB_THREADS = 256;   // one coverage-histogram bin per thread (SweepTally)
+constexpr int TB_REGION_BYTES = 64 * 1024;
+template <int NW>
+constexpr int tb_region_log2() { return __builtin_ctz(TB_REGION_BYTES / (int)sizeof(Slot<NW>)); }
+
+struct TableBuildArgs {
+    BinArgs bins;
+    int sweep, D;     // apply the end-of-pass sweeps (PendingFlush::sweep), delow threshold
+    u64* hist;        // [256] coverage histogram of the swept entries
+    u64* counters;    // C_DISTINCT += keys built; C_CARRY, C_BIN_OVF; C_LINEAR, C_REMOVED; C_SPILLKEYS (k_merge_remnants)
+    u64* spill_list;  // k_merge_remnants: slots of the keys it claimed, swept from this list afterwards (k_sweep_list)
+    u64 spill_cap;
+};
+
+template <int NW>
+__device__ __forceinline__ void slot_load(const Slot<NW>* s, Kmer<NW>& k, u64& pay, u64& rank) {
+    if constexpr (NW == 2) {
+        const U256 v = ld256(s);
+        k.w[0] = v.a; k.w[1] = v.b; pay = v.c; rank = v.d;
+    } else {
+        const U128 x = ldcg128(&s->key[0]), y = ldcg128(&s->key[2]), z = ldcg128(&s->payload);
+        k.w[0] = x.a; k.w[1] = x.b; k.w[2] = y.a; k.w[3] = y.b; pay = z.a; rank = z.b;
+    }
+}
+
+template <int NW>
+__global__ void __launch_bounds__(TB_THREADS) k_table_build(Table<NW> tab, TableBuildArgs a) {
+    constexpr int SW = (int)sizeof(Slot<NW>) / 8;   // words per slot
+    extern __shared__ __align__(16) u64 s_reg[];    // [RS] slots in table format
+    __shared__ SweepTally s_sw;
+    __shared__ unsigned s_new;
+    volatile u64* const vreg = s_reg;
+    const int tid = threadIdx.x;
+    const u32 RS = 1u << a.bins.region_log2;
+    const u64 n_regions = (tab.mask + 1) >> a.bins.region_log2;
+    // a bin overflow leaves partials of some keys on the remnant list, merged after the build: then nothing may be swept here
+    const bool sweep = a.sweep && ldcg64(&a.counters[C_BIN_OVF]) == 0;
+    s_sw.clear();
+    if (tid == 0) s_new = 0;
+    unsigned lin = 0, rem = 0, my_new = 0;
+    for (u64 r = blockIdx.x; r < n_regions; r += gridDim.x) {
+        __syncthreads();   // the previous region is written out
+        for (u32 i = tid; i < RS * SW / 2; i += TB_THREADS) reinterpret_cast<uint4*>(s_reg)[i] = make_uint4(~0u, ~0u, ~0u, ~0u);
+        __syncthreads();
+        Slot<NW>* const g = tab.slots + (r << a.bins.region_log2);
+        const u32 n = min(a.bins.cursor[r], RS);
+        for (u32 i = tid; i < n; i += TB_THREADS) {
+            Kmer<NW> k;
+            u64 pay, rank;
+            slot_load(g + i, k, pay, rank);
+            bool placed = false;
+            // claim: CAS(key0, EMPTY -> w0|BUSY), the other words and {payload, rank}, fence, publish w0; a match merges its partial
+            for (u32 j = (u32)(table_hash(k) & (RS - 1)); j < RS && !placed; j++) {
+                volatile u64* const ks = vreg + (u64)j * SW;
+                u64 k0 = ks[0];
+                if (k0 == EMPTY64) {
+                    k0 = atomicCAS((unsigned long long*)(s_reg + (u64)j * SW), EMPTY64, k.w[0] | BUSY_BIT);
+                    if (k0 == EMPTY64) {
+#pragma unroll
+                        for (int w = 1; w < NW; w++) ks[w] = k.w[w];
+                        ks[NW] = pay;
+                        ks[NW + 1] = rank;
+                        __threadfence_block();
+                        ks[0] = k.w[0];
+                        my_new++;
+                        placed = true;
+                        break;
+                    }
+                }
+                if ((k0 & ~BUSY_BIT) == k.w[0]) {
+                    while (k0 & BUSY_BIT) k0 = ks[0];
+                    bool same = true;
+#pragma unroll
+                    for (int w = 1; w < NW; w++) same = same && ks[w] == k.w[w];
+                    if (same) {
+                        u64 cur = ks[NW];
+                        for (;;) {
+                            const u64 nxt = payload_merge(cur, pay);
+                            if (nxt == cur) break;
+                            const u64 old = atomicCAS((unsigned long long*)(s_reg + (u64)j * SW + NW), cur, nxt);
+                            if (old == cur) break;
+                            cur = old;
+                        }
+                        if (rank < ks[NW + 1]) atomicMin((unsigned long long*)(s_reg + (u64)j * SW + NW + 1), rank);
+                        placed = true;
+                    }
+                }
+            }
+            if (!placed) {   // a carry
+                const u64 c = atomicAdd(&a.counters[C_CARRY], 1ull);
+                if (c < a.bins.remnant_cap) slot_store(reinterpret_cast<Slot<NW>*>(a.bins.remnant) + c, k, pay, rank);
+            }
+        }
+        __syncthreads();   // every entry of the bin is read and placed: its table memory may be overwritten
+        if (sweep)
+            for (u32 j = tid; j < RS; j += TB_THREADS) {
+                u64* const sl = s_reg + (u64)j * SW;
+                if (!(sl[0] == EMPTY64 && sl[1] == EMPTY64)) sl[NW] = sweep_payload(sl[NW], a.D, rem, lin, s_sw.hist);
+            }
+        __syncthreads();
+        for (u32 i = tid; i < RS * SW / 2; i += TB_THREADS) stcg128(reinterpret_cast<U128*>(g) + i, reinterpret_cast<const U128*>(s_reg)[i]);
+    }
+    if (my_new) atomicAdd(&s_new, my_new);
+    s_sw.flush(lin, rem, a.hist, &a.counters[C_LINEAR], &a.counters[C_REMOVED]);   // (synchronises the CTA first)
+    if (tid == 0 && s_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_new);
+}
+
+// The remnant list (bin overflow, then carries) into the finished table with the CAS protocol: a carry's probe continues into the next
+// regions, and a key placed into an empty slot breaks no other key's probe path.  Several entries may hold partials of one key, so a
+// claim merges into the empty slot's {PAYLOAD_FRESH, ~0} like any other writer instead of storing.
+template <int NW>
+__global__ void __launch_bounds__(256) k_merge_remnants(Table<NW> tab, TableBuildArgs a) {
+    __shared__ unsigned s_new;
+    if (threadIdx.x == 0) s_new = 0;
+    __syncthreads();
+    const u64 n = min(ldcg64(&a.counters[C_CARRY]), a.bins.remnant_cap);
+    const Slot<NW>* const list = reinterpret_cast<const Slot<NW>*>(a.bins.remnant);
+    unsigned my_new = 0;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        Kmer<NW> k;
+        u64 pay, rank;
+        slot_load(list + i, k, pay, rank);
+        bool claimed;
+        const u64 idx = table_find_or_claim(tab, k, &claimed);
+        Slot<NW>* const s = tab.slots + idx;
+        slot_merge(s, claimed ? PAYLOAD_FRESH : ldcg64(&s->payload), pay, rank);
+        if (claimed) {
+            my_new++;
+            const u64 sn = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
+            if (sn < a.spill_cap) a.spill_list[sn] = idx;
+        }
+    }
+    if (my_new) atomicAdd(&s_new, my_new);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_new);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -891,7 +1071,9 @@ void EngineT<NW>::skm_init() {
     while ((size_t)skm_part_threads_ * skm_geom_.w * sizeof(u32) > 160 * 1024 && skm_part_threads_ > 32) skm_part_threads_ /= 2;
     const size_t ring = (size_t)skm_part_threads_ * skm_geom_.w * sizeof(u32);
     if (ring > 48 * 1024) PG_CUDA(cudaFuncSetAttribute(k_skm_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
-    PG_CUDA(cudaFuncSetAttribute(k_skm_apply<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)skm_apply_smem<NW>()));
+    PG_CUDA(cudaFuncSetAttribute(k_skm_apply<NW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)skm_apply_smem<NW>()));
+    PG_CUDA(cudaFuncSetAttribute(k_skm_apply<NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)skm_apply_smem<NW>()));
+    PG_CUDA(cudaFuncSetAttribute(k_table_build<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, TB_REGION_BYTES));
     if (prm_.verbose) fprintf(stderr, "[pgb200] aggregated pass 1: %u buckets (%u owned by GPU %d of %d), minimizer length %d, window %d\n", skm_geom_.n_buckets,
                               skm_own_hi_ - skm_own_lo_, prm_.rank, world, skm_geom_.m, skm_geom_.w);
 }
@@ -1126,7 +1308,7 @@ template <int NW>
 void EngineT<NW>::skm_fence() { skm_close_epoch(true); }
 
 template <int NW>
-void EngineT<NW>::skm_launch_apply(const u32* list, u32 n_list, u32* deferred_out) {
+void EngineT<NW>::skm_launch_apply(const u32* list, u32 n_list, u32* deferred_out, bool region) {
     SkmSegList* segs = &skm_scratch_.template as<SkmScratch>()->segs;
     SkmFlushArgs fa;
     fa.world = xa_geom_.world; fa.max_seg = xa_geom_.max_seg; fa.bo_stride = xa_geom_.bo_max + 1; fa.cap_pair = xa_geom_.cap_pair; fa.rec_words = NW + 2;
@@ -1139,22 +1321,19 @@ void EngineT<NW>::skm_launch_apply(const u32* list, u32 n_list, u32* deferred_ou
     aa.segs = segs; aa.bucket_list = list; aa.n_list = n_list; aa.counters = d_cnt_;
     aa.limit = (u64)(SKM_TABLE_LOAD * (double)cap_);
     aa.deferred = deferred_out;
-    aa.sweep = flush_.sweep ? 1 : 0;
-    aa.D = (int)(signed char)prm_.D;   // deLowKmer is a `char` (inc/global.h:67)
-    aa.hist = hist_buf_.template as<u64>();
-    aa.spill_list = spill_list_.template as<u64>();
-    aa.spill_cap = SPILL_CAP;
+    aa.bins = BinArgs{bin_cursor_.template as<u32>(), carry_buf_.p, carry_cap_, region_log2_};
     aa.collapse = SKM_COLLAPSE_AUTO;
     if (const char* e = getenv("PGB200_SKM_COLLAPSE")) {
         if (!strcmp(e, "off")) aa.collapse = SKM_COLLAPSE_OFF;
         else if (!strcmp(e, "on")) aa.collapse = SKM_COLLAPSE_ON;
         else if (strcmp(e, "auto")) throw std::runtime_error("pgb200: PGB200_SKM_COLLAPSE must be auto, on or off");
     }
+    auto kern = region ? k_skm_apply<NW, true> : k_skm_apply<NW, false>;
     int per_sm = 0;
-    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_skm_apply<NW>, SKM_APPLY_THREADS, skm_apply_smem<NW>()));
+    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SKM_APPLY_THREADS, skm_apply_smem<NW>()));
     if (per_sm < 1) per_sm = 1;
     const unsigned blocks = (unsigned)std::min<u64>((u64)n_list, (u64)n_sm_ * per_sm);   // persistent CTAs: as many as are resident
-    if (blocks) k_skm_apply<NW><<<blocks, SKM_APPLY_THREADS, skm_apply_smem<NW>(), st_>>>(tab_, kp_, aa);
+    if (blocks) kern<<<blocks, SKM_APPLY_THREADS, skm_apply_smem<NW>(), st_>>>(tab_, kp_, aa);
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cudaMemcpyAsync(h_outcome_, d_cnt_ + C_XERR, sizeof(FlushOutcome), cudaMemcpyDeviceToHost, st_));
     p1_.launches += 2;
@@ -1167,13 +1346,29 @@ void EngineT<NW>::skm_flush(bool final_of_pass) {
     if (!xa_buf_.p || xa_flushed_epoch_ >= xa_send_epoch_) return;
     skm_flush_complete();
     if (xa_flushed_epoch_ + 1 != xa_send_epoch_) throw std::runtime_error("pgb200: internal: more than one unflushed exchange epoch");
-    create_table_if_needed();
-    // the end-of-pass sweeps ride on this launch when it is the pass so far (PassSweeps)
-    flush_.sweep = pass_sweeps_ == PassSweeps::Untouched && ((signed char)prm_.D <= 0 || final_of_pass);
-    if (flush_.sweep) {
+    // The pass's first launch (no key in the table) builds the table region by region, and the end-of-pass sweeps ride on the build
+    // (PassSweeps); the table memory is then the bins' storage and needs no clear.  Any other launch merges into the table.
+    flush_.region = table_build_region_ && pass_sweeps_ == PassSweeps::Untouched;
+    create_table_if_needed(!flush_.region);
+    flush_.sweep = flush_.region && ((signed char)prm_.D <= 0 || final_of_pass);
+    if (flush_.region) {
+        int rl = tb_region_log2<NW>();
+        if (const char* e = getenv("PGB200_TABLE_REGION")) {   // slots per region (a power of two; tests use tiny regions for carries)
+            const u64 v = strtoull(e, nullptr, 0);
+            if (v < 1 || (v & (v - 1)) || v > (1ull << rl)) throw std::runtime_error("pgb200: PGB200_TABLE_REGION must be a power of two up to the 64 KB region");
+            rl = __builtin_ctzll(v);
+        }
+        while ((1ull << rl) > cap_) rl--;
+        region_log2_ = rl;
+        bin_cursor_.ensure((cap_ >> rl) * sizeof(u32));
+        carry_cap_ = std::max<u64>(cap_ / 64, 1ull << 16);
+        if (const char* e = getenv("PGB200_TABLE_REMNANT_CAP")) carry_cap_ = strtoull(e, nullptr, 0);
+        carry_buf_.ensure(carry_cap_ * sizeof(Slot<NW>));
         hist_buf_.ensure(256 * sizeof(u64));
         spill_list_.ensure(SPILL_CAP * sizeof(u64));
+        PG_CUDA(cudaMemsetAsync(bin_cursor_.p, 0, (cap_ >> rl) * sizeof(u32), st_));
         PG_CUDA(cudaMemsetAsync(d_cnt_ + C_SPILLKEYS, 0, sizeof(u64), st_));
+        PG_CUDA(cudaMemsetAsync(d_cnt_ + C_CARRY, 0, 2 * sizeof(u64), st_));   // C_CARRY, C_BIN_OVF
         PG_CUDA(cudaMemsetAsync(hist_buf_.p, 0, 256 * sizeof(u64), st_));
         PG_CUDA(cudaMemsetAsync(d_cnt_ + C_LINEAR, 0, 2 * sizeof(u64), st_));
     }
@@ -1181,9 +1376,33 @@ void EngineT<NW>::skm_flush(bool final_of_pass) {
     PG_CUDA(cudaMemsetAsync(d_cnt_ + C_SKM_STAGED, 0, 2 * sizeof(u64), st_));
     flush_.half = (int)(xa_flushed_epoch_ % SKM_ARENA_HALVES);
     PG_CUDA(cudaEventRecord(ev_flush_begin_, st_));
-    skm_launch_apply(nullptr, skm_own_hi_ - skm_own_lo_, skm_deferred_[0].template as<u32>());
+    skm_launch_apply(nullptr, skm_own_hi_ - skm_own_lo_, skm_deferred_[0].template as<u32>(), flush_.region);
+    if (flush_.region) table_build_launch();
     PG_CUDA(cudaEventRecord(ev_flush_, st_));
     flush_.pending = true;
+}
+
+// k_table_build + k_merge_remnants behind the region-mode aggregation launch (inside its timing events)
+template <int NW>
+void EngineT<NW>::table_build_launch() {
+    TableBuildArgs b;
+    b.bins = BinArgs{bin_cursor_.template as<u32>(), carry_buf_.p, carry_cap_, region_log2_};
+    b.sweep = flush_.sweep ? 1 : 0;
+    b.D = (int)(signed char)prm_.D;   // deLowKmer is a `char` (inc/global.h:67)
+    b.hist = hist_buf_.template as<u64>();
+    b.counters = d_cnt_;
+    b.spill_list = spill_list_.template as<u64>();
+    b.spill_cap = SPILL_CAP;
+    const size_t smem = sizeof(Slot<NW>) << region_log2_;
+    int per_sm = 0;
+    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_table_build<NW>, TB_THREADS, smem));
+    if (per_sm < 1) per_sm = 1;
+    k_table_build<NW><<<(unsigned)std::min<u64>(cap_ >> region_log2_, (u64)n_sm_ * per_sm), TB_THREADS, smem, st_>>>(tab_, b);
+    PG_CUDA(cudaGetLastError());
+    k_merge_remnants<NW><<<n_sm_ * 4, 256, 0, st_>>>(tab_, b);
+    PG_CUDA(cudaGetLastError());
+    table_dirty_ = false;   // every slot is written
+    p1_.launches += 2;
 }
 
 template <int NW>
@@ -1196,6 +1415,32 @@ void EngineT<NW>::skm_flush_complete() {
     int launches = 1, which = 0;
     FlushOutcome out = *h_outcome_;
     if (out.xerr) throw std::runtime_error("pgb200: too many segments in one exchange epoch (flush more often)");
+    if (flush_.region) {
+        u64 rc[2];   // C_CARRY, C_BIN_OVF
+        PG_CUDA(cudaMemcpy(rc, d_cnt_ + C_CARRY, sizeof rc, cudaMemcpyDeviceToHost));
+        const bool redo = rc[0] > carry_cap_;
+        if (prm_.verbose)
+            fprintf(stderr, "[pgb200] region build: %llu regions of %u slots, bin overflow %llu, carries %llu, remnant list %llu of %llu%s\n",
+                    (unsigned long long)(cap_ >> region_log2_), 1u << region_log2_, (unsigned long long)rc[1], (unsigned long long)(rc[0] - rc[1]),
+                    (unsigned long long)rc[0], (unsigned long long)carry_cap_, redo ? ": full, the launch runs again in merge mode" : "");
+        if (rc[1] && pass_sweeps_ == PassSweeps::Fused) pass_sweeps_ = PassSweeps::Plain;   // the build swept nothing (k_table_build)
+        if (redo) {
+            // entries were dropped: the same records again, the classic way, into a cleared table (the launch found it empty)
+            pass_sweeps_ = PassSweeps::Plain;
+            PG_CUDA(cudaMemsetAsync(tab_buf_.p, 0xFF, cap_ * sizeof(Slot<NW>), st_));
+            PG_CUDA(cudaMemsetAsync(d_cnt_ + C_DISTINCT, 0, sizeof(u64), st_));
+            PG_CUDA(cudaMemsetAsync(d_cnt_ + C_SKM_STAGED, 0, 2 * sizeof(u64), st_));
+            PG_CUDA(cudaEventRecord(ev_flush_begin_, st_));
+            skm_launch_apply(nullptr, skm_own_hi_ - skm_own_lo_, skm_deferred_[0].template as<u32>(), false);
+            PG_CUDA(cudaEventRecord(ev_flush_, st_));
+            PG_CUDA(cudaEventSynchronize(ev_flush_));
+            float ms2;
+            PG_CUDA(cudaEventElapsedTime(&ms2, ev_flush_begin_, ev_flush_));
+            ms += ms2;
+            launches++;
+            out = *h_outcome_;
+        }
+    }
     while (out.defer) {
         // buckets whose worst case did not fit the table: grow so that (at least) the largest one fits, run them again
         read_counters();
@@ -1203,7 +1448,7 @@ void EngineT<NW>::skm_flush_complete() {
             throw std::runtime_error("pgb200: k-mer table cannot grow further (out of HBM); use more GPUs");
         if (pass_sweeps_ == PassSweeps::Fused) pass_sweeps_ = PassSweeps::Plain;   // the spill list holds slots of the table just replaced
         PG_CUDA(cudaEventRecord(ev_flush_begin_, st_));
-        skm_launch_apply(skm_deferred_[which].template as<u32>(), (u32)out.defer, skm_deferred_[which ^ 1].template as<u32>());
+        skm_launch_apply(skm_deferred_[which].template as<u32>(), (u32)out.defer, skm_deferred_[which ^ 1].template as<u32>(), false);
         PG_CUDA(cudaEventRecord(ev_flush_, st_));
         PG_CUDA(cudaEventSynchronize(ev_flush_));
         float ms2;
@@ -1276,7 +1521,8 @@ void EngineT<NW>::skm_reset() {
     template void EngineT<NW>::skm_fence();                                  \
     template void EngineT<NW>::skm_close_epoch(bool);                        \
     template void EngineT<NW>::skm_flush_complete();                         \
-    template void EngineT<NW>::skm_launch_apply(const u32*, u32, u32*);      \
+    template void EngineT<NW>::skm_launch_apply(const u32*, u32, u32*, bool); \
+    template void EngineT<NW>::table_build_launch();                         \
     template u64 EngineT<NW>::skm_room_estimate(u64);                        \
     template void EngineT<NW>::skm_flush(bool);                              \
     template void EngineT<NW>::skm_reset();
