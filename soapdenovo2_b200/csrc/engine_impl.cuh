@@ -1,5 +1,6 @@
 // engine_impl.cuh -- EngineT<NW>: device state + phase methods; the methods are defined across decode.cu, pass1.cu, skm.cu,
-// layout.cu, tips.cu, edges.cu, pass2.cu and explicitly instantiated for NW = 2 (K <= 63) and NW = 4 (K <= 127).
+// skm_apply.cu, table_build.cu, layout.cu, tips.cu, edges.cu, pass2.cu and explicitly instantiated for NW = 2 (K <= 63) and NW = 4
+// (K <= 127).
 #pragma once
 #include "engine.h"
 #include "kmer.cuh"
@@ -89,10 +90,10 @@ static_assert(C_INSTANCES == C_DISTINCT + 1 && C_KEPT == C_DISTINCT + 2, "absorb
 
 // Whether the end-of-pass sweeps (K4) already ran inside this pass's aggregation launch.  They can, when the launch is the pass so far (no
 // key in the table, no launch and no per-instance insert before it): such a launch builds the table region by region (k_table_build,
-// skm.cu), every entry is final when its region is written, and one pass over the table is saved.  Without -d the sweeps only SET flags
-// that k_sweep recomputes, so the build may do them speculatively; with -d the link counters are zeroed for good, so the launch must be
-// known to be the last of the pass (finish_pass1 on one GPU).  Whatever touches the table afterwards -- another launch, a per-instance
-// insert, a table growth, a bin overflow, more carries than the spill list holds -- makes the result Plain.
+// table_build.cu), every entry is final when its region is written, and one pass over the table is saved.  Without -d the sweeps only
+// SET flags that k_sweep recomputes, so the build may do them speculatively; with -d the link counters are zeroed for good, so the
+// launch must be known to be the last of the pass (finish_pass1 on one GPU).  Whatever touches the table afterwards -- another launch,
+// a per-instance insert, a table growth, a bin overflow, more carries than the spill list holds -- makes the result Plain.
 //   Untouched  no aggregation launch and no per-instance insert since reset_pass1
 //   Fused      this pass's only launch was a region build that applied the sweeps, and they still hold: sweeps() sweeps the carries only
 //   Plain      anything else: sweeps() runs k_sweep over the whole table
@@ -122,6 +123,8 @@ struct PendingFlush {
     bool sweep = false;   // ... and the build applied the end-of-pass sweeps
     int half = 0;         // the arena half it reads
 };
+
+struct BinArgs;   // table_build.cuh
 
 template <int NW>
 class EngineT : public IEngine {
@@ -192,7 +195,8 @@ public:
     // pass 1, per-instance insert (pass1.cu): PGB200_SKM=0, single GPU only -- the second exact path the parity tests compare with
     void chop_insert_chunk(const ReadChunk& ch);
     void check_format_counter();
-    // pass 1, aggregated (skm.cu): super-k-mer records scattered into the owners' arenas, one table update per DISTINCT k-mer
+    // pass 1, aggregated: super-k-mer records scattered into the owners' arenas, one table update per DISTINCT k-mer
+    // ... the exchange (skm.cu)
     int skm_mode_ = -1;          // -1: aggregated for device-resident text, per-instance inserts for host text; 0 / 1: forced (PGB200_SKM)
     int skm_flush_every_ = -1;   // single GPU: aggregate every n chunks (-1: host text whenever the insert stream is idle, device text only when the arena is full)
     SkmGeom skm_geom_;
@@ -200,50 +204,54 @@ public:
     int skm_own_shift_ = -1;
     int skm_part_threads_ = 128;
     DevBuf skm_cnt_, skm_segoff_, skm_cursor_, skm_scan_, skm_side_;
-    DevBuf skm_scratch_;               // SkmScratch (skm.cu): the exchange's device-side cursors, scan total and segment list
-    DevBuf skm_deferred_[2];           // deferred buckets of an aggregation launch, read by the re-run that writes the other list
+    DevBuf skm_scratch_;               // SkmScratch (skm.cu): the exchange's device-side cursors and scan total
     // the exchange arena: [SKM_ARENA_HALVES][nseg | ring | offsets | world x cap_pair records]; xa_peer_[o] = owner o's arena as mapped here
     SkmArenaGeom xa_geom_;
     DevBuf xa_buf_;
     std::vector<void*> xa_peer_, xa_ipc_opened_;
     u64 xa_send_epoch_ = 0, xa_flushed_epoch_ = 0;
     u32 xa_seg_idx_ = 0;
-    PendingFlush flush_;
-    PassSweeps pass_sweeps_ = PassSweeps::Untouched;
-    DevBuf spill_list_;                // slots of the keys a Fused launch stored unswept (the region build's carries)
-    static constexpr u64 SPILL_CAP = 1ull << 22;
-    // the region build (PGB200_TABLE_BUILD=region, the default; merge: every launch merges into the global table with the CAS protocol)
-    bool table_build_region_ = true;
-    int region_log2_ = 0;              // slots per region (and bin capacity) = 2^region_log2_
-    DevBuf bin_cursor_;                // [regions] u32: entries the aggregation stored in each bin
-    DevBuf carry_buf_;                 // remnant list: entries past their bin's capacity, then the build's carries (Slot<NW> format)
-    u64 carry_cap_ = 0;
-    void table_build_launch();
-    Pinned<FlushOutcome> h_outcome_;   // as of the end of the last aggregation launch
-    Event ev_flush_begin_, ev_flush_;
-    void skm_close_epoch(bool hard);
-    void skm_flush_complete();
-    void skm_launch_apply(const u32* list, u32 n_list, u32* deferred_out, bool region);
     std::vector<u64> xa_reads_cum_;   // reads fed in this epoch after 0, 1, 2, ... chunks (the fill known to the host lags behind)
-    u64 skm_room_estimate(u64 n_rec);
     bool xa_dirty_ = false;
     void skm_init();
     void xchg_default_setup();
-    void skm_send_args(void* out_args, int half);
+    u64 skm_room_estimate(u64 n_rec);
     void skm_make_room(u64 n_rec, bool host_text);
     void skm_feed_chunk(size_t ci);
+    void skm_close_epoch(bool hard);
     void skm_fence();
-    void skm_flush(bool final_of_pass = false);
     void skm_reset();
-public:
     void xchg_setup(uint64_t cap_records) override;
     void xchg_export(void* handle64) override;
     void xchg_import(int peer, const void* handle64) override;
     void* xchg_base() override;
     void xchg_import_ptr(int peer, int peer_device, void* base) override;
     void xchg_fence() override { skm_fence(); }
-    void flush() override { skm_flush(); }
     bool xchg_room(uint64_t n_rec) override;
+    // ... the bucket aggregation (skm_apply.cu)
+    DevBuf skm_segs_;                  // SkmSegList (skm_apply.cu): the segments an aggregation launch reads
+    DevBuf skm_deferred_[2];           // deferred buckets of an aggregation launch, read by the re-run that writes the other list
+    PendingFlush flush_;
+    PassSweeps pass_sweeps_ = PassSweeps::Untouched;
+    Pinned<FlushOutcome> h_outcome_;   // as of the end of the last aggregation launch
+    Event ev_flush_begin_, ev_flush_;
+    void skm_launch_apply(const u32* list, u32 n_list, u32* deferred_out, bool region);
+    void skm_flush(bool final_of_pass = false);
+    void skm_flush_complete();
+    void flush() override { skm_flush(); }
+    // ... the region build (table_build.cu; PGB200_TABLE_BUILD=region, the default; merge: every launch merges into the global table
+    // with the CAS protocol)
+    bool table_build_region_ = true;
+    int region_log2_ = 0;              // slots per region (and bin capacity) = 2^region_log2_
+    DevBuf bin_cursor_;                // [regions] u32: entries the aggregation stored in each bin
+    DevBuf carry_buf_;                 // remnant list: entries past their bin's capacity, then the build's carries (Slot<NW> format)
+    u64 carry_cap_ = 0;
+    DevBuf spill_list_;                // slots of the keys a Fused launch stored unswept (the region build's carries)
+    static constexpr u64 SPILL_CAP = 1ull << 22;
+    BinArgs bin_args() const;          // where a region-mode aggregation launch stores its aggregates (table_build.cuh)
+    void table_build_prepare();
+    void table_build_launch();
+    bool table_build_redo();
     void absorb(IEngine* other) override;
 
     // helpers

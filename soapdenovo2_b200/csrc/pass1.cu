@@ -1,5 +1,5 @@
 // pass1.cu -- pass 1 of pregraph on the GPU: the per-instance insert (the second exact insert path; the default is the aggregated
-// one in skm.cu), the table management, and the per-entry sweeps (delow, mark-linear, kmerFreq histogram).
+// one in skm.cu and skm_apply.cu), the table management, and the per-entry sweeps (delow, mark-linear, kmerFreq histogram).
 //
 // Replaces (reference file:line, standardPregraph/):
 //   K2  chopKmer4read (prlHashReads.c:163-259)                                              -> k_chop_insert (rolling part)
@@ -20,7 +20,7 @@ namespace pgb {
 // (SURVEY.md A.2) and apply the instance to the table.  rank = (read ordinal << 16) | position.
 // This kernel sits on the rate of random DRAM slot updates: one slot
 // read + write-back per k-mer INSTANCE.  It is kept as the independent second implementation that every parity test also runs
-// (PGB200_SKM=0); the product default touches HBM once per DISTINCT k-mer (skm.cu).
+// (PGB200_SKM=0); the product default touches HBM once per DISTINCT k-mer (skm_apply.cu).
 constexpr int INS_THREADS = 256;
 #ifndef INS_MIN_BLOCKS
 #define INS_MIN_BLOCKS 5

@@ -1,4 +1,5 @@
-// skm.cuh -- super-k-mer records: the unit of the aggregated pass 1 and of the multi-GPU exchange (host + device logic; skm.cu).
+// skm.cuh -- super-k-mer records: the unit of the aggregated pass 1 and of the multi-GPU exchange (host + device logic; skm.cu,
+// skm_apply.cu).
 //
 // Why: a random update of an HBM-resident slot costs one DRAM read + one write-back whatever instruction performs it, and a
 // per-instance insert (k_chop_insert, pass1.cu) pays that once per k-mer INSTANCE.
@@ -25,6 +26,12 @@ constexpr int SKM_MAX_RUN = 32;      // k-mers per record: 1 + n + K bases must 
 constexpr int SKM_MAX_M = 15;        // minimizer length (2m bits must fit in 32)
 constexpr int SKM_MAX_BUCKET_BITS = 26;
 constexpr int SKM_MAX_SEGS = 128;    // segments (fed chunks, over all senders) one aggregation launch can read
+constexpr int SKM_MAXW = 16;         // GPUs of one box
+// Slots of a bucket's shared-memory table in the aggregation (k_skm_apply); skm_init sizes the buckets from it
+#ifndef SKM_LOG2_SLOTS
+#define SKM_LOG2_SLOTS 10
+#endif
+constexpr int SKM_SLOTS = 1 << SKM_LOG2_SLOTS;
 
 struct SkmGeom {
     int K = 0, m = 0, w = 0;   // w = K - m + 1 m-mers per k-mer
@@ -357,7 +364,7 @@ PG_HD SkmInst<NW> skm_instance_rec(const KParams<NW>& kp, u64 hdr, const u64 (&x
     return r;
 }
 
-// The same instances from a record staged in shared memory (skm.cu stages a window of records at a time).  Once per record the
+// The same instances from a record staged in shared memory (skm_apply.cu stages a window of records at a time).  Once per record the
 // aggregation writes rv[0..NW]: the record's bases 0 .. n+K-1 in REVERSE order, base n+K-1 at bit 0 and base p at bit 2(n+K-1-p)
 // (the right neighbour of the last k-mer is dropped).  Forward k-mer t is then rv >> 2(n-1-t), a shift by less than 64 bits like the
 // one that gives the reverse complement from the record words: no per-instance reverse complement.
@@ -429,7 +436,7 @@ PG_HD SkmInst<NW> skm_instance_staged(const KParams<NW>& kp, u64 hdr, const u64*
 // Two records with equal header bits 0-7 (n, last, has_prev) and equal base words make the same k-mer instances (skm_make_rec zeroes
 // every base past the meaningful ones): only the ranks differ.  Copy r's k-mer t has rank (ord_r << 16) | (start_r + t), so the
 // smallest rank over the copies is that of the copy with the smallest header (the low 8 bits being equal, headers order by
-// (ordinal, start)).  The aggregation (skm.cu) therefore keeps each distinct record once, with the minimum header and a count c,
+// (ordinal, start)).  The aggregation (skm_apply.cu) therefore keeps each distinct record once, with the minimum header and a count c,
 // and applies its k-mers with payload_apply_n(.., c): the same {payload, rank} per k-mer as every copy expanded on its own.
 template <int NW>
 PG_HD bool skm_rec_same(const u64* a, const u64* b) {
@@ -471,24 +478,6 @@ PG_HD u32 skm_slot_hash(const Kmer<NW>& k, int log2_slots) {
     x ^= x >> 31;
     x *= 0x9E3779B97F4A7C15ull;
     return (u32)(x >> (64 - log2_slots));
-}
-
-// Two partial results for the same k-mer -> the result of all their instances together.  `g` may be PAYLOAD_FRESH (slot claimed, no
-// instance yet); `a` holds at least one instance.  Every instance has a neighbour on at least one side (reads are >= K+1 long), so
-// cov counts instances (newhash.c:74-106, 123-140) and the fields simply add with their saturation; `single` survives only when the
-// total is one instance, i.e. never when both sides are non-empty.
-PG_HD u64 payload_merge(u64 g, u64 a) {
-    if (g == PAYLOAD_FRESH) return a;
-    u64 r = 0;
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-        unsigned l = pl_l(g, c) + pl_l(a, c), q = pl_r(g, c) + pl_r(a, c);
-        r |= (u64)(l > 63 ? 63 : l) << (6 * c);
-        r |= (u64)(q > 63 ? 63 : q) << (PL_R_SHIFT + 6 * c);
-    }
-    unsigned cv = pl_cov(g) + pl_cov(a);
-    r |= (u64)(cv > 255 ? 255 : cv) << PL_COV_SHIFT;
-    return r;
 }
 
 // ---------------------------------------------------------------- exchange arena (one per GPU; see skm.cu)

@@ -62,7 +62,7 @@ PG_HD u64 payload_apply(u64 p, unsigned left, unsigned right) {
     return (p + inc) & ~PL_SINGLE;
 }
 // c identical instances applied at once: equals c calls of payload_apply (c >= 1), and IS payload_apply when c == 1.  The aggregation
-// applies each k-mer of a record that occurs c times in its bucket this way (skm.cu).
+// applies each k-mer of a record that occurs c times in its bucket this way (skm_apply.cu).
 PG_HD u64 payload_apply_n(u64 p, unsigned left, unsigned right, unsigned c) {
     if (c == 1) return payload_apply(p, left, right);
     if (p == PAYLOAD_FRESH) { p = payload_apply(p, left, right); c--; }
@@ -84,9 +84,27 @@ PG_HD u64 payload_apply_n(u64 p, unsigned left, unsigned right, unsigned c) {
     return p & ~PL_SINGLE;
 }
 
+// Two partial results for the same k-mer -> the result of all their instances together.  `g` may be PAYLOAD_FRESH (slot claimed, no
+// instance yet); `a` holds at least one instance.  Every instance has a neighbour on at least one side (reads are >= K+1 long), so
+// cov counts instances (newhash.c:74-106, 123-140) and the fields simply add with their saturation; `single` survives only when the
+// total is one instance, i.e. never when both sides are non-empty.
+PG_HD u64 payload_merge(u64 g, u64 a) {
+    if (g == PAYLOAD_FRESH) return a;
+    u64 r = 0;
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+        unsigned l = pl_l(g, c) + pl_l(a, c), q = pl_r(g, c) + pl_r(a, c);
+        r |= (u64)(l > 63 ? 63 : l) << (6 * c);
+        r |= (u64)(q > 63 ? 63 : q) << (PL_R_SHIFT + 6 * c);
+    }
+    unsigned cv = pl_cov(g) + pl_cov(a);
+    r |= (u64)(cv > 255 ? 255 : cv) << PL_COV_SHIFT;
+    return r;
+}
+
 // The per-entry sweeps of pass 1's end (K4): delow (thread_delow: zero every link counter <= D, deleted = 1 if nothing is left), mark
 // (thread_mark: linear = 1 iff exactly one non-zero left and one non-zero right link, NO deleted check there), histogram of cov.
-// Used by k_sweep (pass1.cu) and, fused, by the aggregation kernel's flush (skm.cu).  The linear flag is recomputed, not inherited.
+// Used by k_sweep (pass1.cu) and, fused, by the region build (table_build.cu).  The linear flag is recomputed, not inherited.
 #if defined(__CUDACC__)
 __device__ __forceinline__ u64 sweep_payload(u64 p, int D, unsigned& rem, unsigned& lin, unsigned* s_hist) {
     p &= ~PL_LINEAR;
@@ -180,6 +198,35 @@ PG_D u64 ldacq64(const void* p) {
     return r;
 }
 PG_D void stcg128(void* p, U128 v) { asm volatile("st.global.cg.v2.u64 [%0], {%1,%2};" ::"l"(p), "l"(v.a), "l"(v.b) : "memory"); }
+// A record goes out with as few stores as possible: over NVLink every store is a packet.  sm_90's widest global store is 128 bits, so
+// a 32-byte record is two 16-byte stores to the same sector.
+PG_D void st256(u64* dst, u64 a, u64 b, u64 c, u64 d) {
+    asm volatile("st.global.v2.u64 [%0], {%1,%2};\n\t"
+                 "st.global.v2.u64 [%0+16], {%3,%4};" ::"l"(dst), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
+}
+
+// One whole slot {key, payload, rank} with 16-byte stores (fire and forget)
+template <int NW>
+PG_D void slot_store(Slot<NW>* s, const Kmer<NW>& k, u64 pay, u64 rank) {
+    u64* d = reinterpret_cast<u64*>(s);
+    if (NW == 2) {
+        st256(d, k.w[0], k.w[1], pay, rank);
+    } else {
+        stcg128(d, U128{k.w[0], k.w[1]});
+        stcg128(d + 2, U128{k.w[2], k.w[3]});
+        stcg128(d + 4, U128{pay, rank});
+    }
+}
+template <int NW>
+PG_D void slot_load(const Slot<NW>* s, Kmer<NW>& k, u64& pay, u64& rank) {
+    if constexpr (NW == 2) {
+        const U256 v = ld256(s);
+        k.w[0] = v.a; k.w[1] = v.b; pay = v.c; rank = v.d;
+    } else {
+        const U128 x = ldcg128(&s->key[0]), y = ldcg128(&s->key[2]), z = ldcg128(&s->payload);
+        k.w[0] = x.a; k.w[1] = x.b; k.w[2] = y.a; k.w[3] = y.b; pay = z.a; rank = z.b;
+    }
+}
 
 // Find-or-claim the slot of key k.  Returns the slot index; *claimed = true if this call inserted the key.
 template <int NW>
@@ -305,6 +352,36 @@ PG_D bool table_insert<2>(const Table<2>& t, const Kmer<2>& k, unsigned left, un
     if (idx_out) *idx_out = idx;
     slot_apply(s, cur.a, cur.b, left, right, rank, c);
     return claimed;
+}
+
+// A partial aggregate into an entry whose payload word was `cur` when read: the 64-bit CAS + atomicMin protocol every writer uses,
+// on the {payload, rank} words of a table slot or of a slot of a region built in shared memory
+PG_D void slot_merge(u64* pay, u64* rnk, u64 cur, u64 agg, u64 rank) {
+    for (;;) {
+        u64 nxt = payload_merge(cur, agg);
+        if (nxt == cur) break;
+        u64 old = atomicCAS(pay, cur, nxt);
+        if (old == cur) break;
+        cur = old;
+    }
+    atomicMin(rnk, rank);
+}
+
+// One aggregated k-mer -> the global table (merge mode, or a launch after the pass's first).  A k-mer lives in exactly one bucket and a
+// bucket is aggregated by one CTA at a time, so when this call CLAIMS the slot nobody else can be touching its {payload, aux} words:
+// they are written with one plain 16-byte store (probe load -> claim CAS -> store: two dependent memory round trips per new key).  A key
+// that already exists (earlier epoch, or a lane of this bucket spilled the key) is merged with slot_merge.
+template <int NW>
+PG_D bool table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank) {
+    bool claimed;
+    u64 idx = table_find_or_claim(t, k, &claimed);
+    Slot<NW>* s = t.slots + idx;
+    if (claimed) {
+        stcg128(&s->payload, U128{agg, rank});
+        return true;
+    }
+    slot_merge(&s->payload, &s->aux, ldcg64(&s->payload), agg, rank);
+    return false;
 }
 
 template <int NW>

@@ -1,4 +1,4 @@
-// Host-side check of the record collapse of the aggregated pass 1 (skm.cu: k_skm_apply, skm_dedup_insert), compiled with nvcc and
+// Host-side check of the record collapse of the aggregated pass 1 (skm_apply.cu: k_skm_apply, skm_dedup_insert), compiled with nvcc and
 // run on the CPU by tests/test_skm_collapse_host.py.
 //   * payload_apply_n(p, left, right, c) equals c calls of payload_apply for every left/right in 0..4 and c in 1..600, from the fresh
 //     state, saturated links and coverage, `single`, and random payloads;

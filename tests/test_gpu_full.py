@@ -81,7 +81,7 @@ def test_multilib_k63_small_chunks(tmp_path):
 
 
 def test_multilib_k63_aggregated_pass1(tmp_path):
-    """The same multi-library case with pass 1 forced through the aggregated path (super-k-mer records, skm.cu), several chunks."""
+    """The same multi-library case with pass 1 forced through the aggregated path (super-k-mer records, skm.cu and skm_apply.cu), several chunks."""
     cfg = synth.scenario_multilib(str(tmp_path))
     ref, gpu = str(tmp_path / "ref"), str(tmp_path / "gpu")
     _oracle(0, cfg, ref, 63, 8, ("-a", "1", "-R"))

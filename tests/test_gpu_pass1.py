@@ -18,7 +18,7 @@ def _build():
 @pytest.fixture(params=["direct", "aggregated"], autouse=True)
 def _insert_mode(request, monkeypatch):
     """Every case runs twice: per-instance inserts (k_chop_insert, the default for host text) and the aggregated pass 1 (super-k-mer
-    records, skm.cu: the default for device-resident text and the only path across GPUs), both forced through PGB200_SKM."""
+    records, skm.cu and skm_apply.cu: the default for device-resident text and the only path across GPUs), both forced through PGB200_SKM."""
     monkeypatch.setenv("PGB200_SKM", "0" if request.param == "direct" else "1")
 
 

@@ -1,5 +1,5 @@
 """GPU parity, pass 1, on reads made of exact copies: every super-k-mer record of the aggregated pass 1 occurs tens to hundreds of
-times in its bucket, so the aggregation collapses them into distinct records with counts (skm.cu, k_skm_apply) and applies each k-mer
+times in its bucket, so the aggregation collapses them into distinct records with counts (skm_apply.cu, k_skm_apply) and applies each k-mer
 once per distinct record, weighted by its count.  Counts past 255 saturate the coverage and past 63 the links.  The .kmerFreq and
 the full node table dump must equal the C model's, with the default bucket count and with ONE bucket (the distinct-record buffer
 drains many times per window and every k-mer past the shared-memory table goes to the global table with its weight)."""
