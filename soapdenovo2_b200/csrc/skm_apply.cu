@@ -31,11 +31,10 @@ constexpr int SKM_SOFT_LIMIT = SKM_SLOTS - SKM_APPLY_THREADS - 64;   // claims s
 
 // ------------------------------------------------------------------------------------------------ aggregation
 // Shared-memory table of one bucket, structure of arrays: key words [NW][S], payload [S], rank [S], claim list [S] (u16).
-// Claim protocol: CAS(key0, EMPTY -> w0|BUSY), write the other key words, fence, store w0.  Empty slots hold {PAYLOAD_FRESH, ~0} in
-// their payload / rank words, so the claimer records its own instance together with the lanes that found the key (one update path).
-// A thread that meets a BUSY key0 whose other bits match waits for the publication (independent thread scheduling: the claimer makes
-// progress even inside the same warp).  The claimer also appends the slot to the claim list (the flush walks the list, not the
-// table).  (Prefetching the k-mer's home slot of the GLOBAL table into L2 at claim time measured no difference and was dropped.)
+// Claim protocol: smem_find_or_claim.  Empty slots hold {PAYLOAD_FRESH, ~0} in their payload / rank words, so the claimer records its
+// own instance together with the lanes that found the key (one update path).  The claimer also appends the slot to the claim list (the
+// flush walks the list, not the table).  (Prefetching the k-mer's home slot of the GLOBAL table into L2 at claim time measured no
+// difference and was dropped.)
 // S slots (any size: the slot index is a multiply-shift range reduction of a 32-bit hash), claims stop at LIMIT so that the
 // table can never fill up completely whatever the number of concurrent claimers; LT = type of the claim-list entries.
 template <int NW, int S, int LIMIT, class LT>
@@ -50,49 +49,18 @@ struct SmemTable {
     // instance TOGETHER (without the barrier the lanes that match on their first probe run the long update on their own while the
     // others keep probing: the update code then executes several times per step with a few active lanes each).
     // find(): 1 = key present at idx (found, or claimed by this lane just now), 3 = no room (caller spills)
-    __device__ __forceinline__ int find(const Table<NW>& tab, const Kmer<NW>& k, u32& idx) const {
+    __device__ __forceinline__ int find(const Kmer<NW>& k, u32& idx) const {
         idx = (u32)(((u64)skm_slot_hash(k, 32) * (u64)S) >> 32);
-        volatile u64* vkey = key;
-        for (int probe = 0; probe < S; probe++) {
-            u64 k0 = vkey[idx];
-            if (k0 == EMPTY64) {
-                if (*(volatile u32*)count >= (u32)LIMIT) return 3;
-                u64 old = atomicCAS(&key[idx], EMPTY64, k.w[0] | BUSY_BIT);
-                if (old == EMPTY64) {
-#pragma unroll
-                    for (int w = 1; w < NW; w++) vkey[w * S + idx] = k.w[w];
-                    __threadfence_block();
-                    vkey[idx] = k.w[0];
-                    const u32 n = atomicAdd(count, 1u);
-                    list[n] = (LT)idx;
-                    return 1;   // an empty slot holds {PAYLOAD_FRESH, ~0}: the claimer records its instance with everybody else in apply()
-                }
-                k0 = old;
-            }
-            if ((k0 & ~BUSY_BIT) == k.w[0]) {
-                while (k0 & BUSY_BIT) k0 = vkey[idx];
-                bool same = true;
-#pragma unroll
-                for (int w = 1; w < NW; w++) same = same && vkey[w * S + idx] == k.w[w];
-                if (same) return 1;
-            }
-            idx = idx + 1 == (u32)S ? 0u : idx + 1;
-        }
-        return 3;
+        // an empty slot holds {PAYLOAD_FRESH, ~0}: the claimer records its instance with everybody else in apply()
+        return smem_find_or_claim<NW, true>(key, 1, S, S, k, idx, [&] { return *(volatile u32*)count < (u32)LIMIT; }, [](u32) {},
+                                            [&](u32 j, bool claimed) {
+                                                if (claimed) list[atomicAdd(count, 1u)] = (LT)j;
+                                            }) ? 1 : 3;
     }
     // c identical instances
     __device__ __forceinline__ void apply(u32 idx, unsigned left, unsigned right, u64 rank, unsigned c) const {
-        volatile u64* vpay = pay;
-        volatile u64* vrnk = rnk;
-        u64 cur = vpay[idx];
-        for (;;) {
-            u64 nxt = payload_apply_n(cur, left, right, c);
-            if (nxt == cur) break;
-            u64 old = atomicCAS(&pay[idx], cur, nxt);
-            if (old == cur) break;
-            cur = old;
-        }
-        if (rank < vrnk[idx]) atomicMin(&rnk[idx], rank);
+        payload_fold(&pay[idx], ((volatile u64*)pay)[idx], [=](u64 p) { return payload_apply_n(p, left, right, c); });
+        rank_min(&rnk[idx], rank, rank < ((volatile u64*)rnk)[idx]);
     }
 };
 
@@ -471,7 +439,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
                     SKM_ACC(1, t_inst);
                     SKM_T0(t_find);
                     u32 slot;
-                    const int state = st.find(tab, in.canon, slot);
+                    const int state = st.find(in.canon, slot);
                     __syncwarp(has_mask);   // the lanes re-join before the counter update (see SmemTable)
                     SKM_ACC(2, t_find);
                     SKM_T0(t_upd);
@@ -485,7 +453,7 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
                         if constexpr (REGION) {
                             bin_store(tab, a.bins, a.counters, in.canon, payload_apply_n(PAYLOAD_FRESH, in.left, in.right, c), rank);
                             atomicAdd(&s_new, 1u);
-                        } else if (table_insert(tab, in.canon, in.left, in.right, rank, nullptr, c)) {
+                        } else if (table_insert(tab, in.canon, in.left, in.right, rank, c)) {
                             atomicAdd(&s_new, 1u);
                         }
                         SKM_ACC(4, t_upd);
@@ -564,7 +532,9 @@ __global__ void __launch_bounds__(SKM_APPLY_THREADS, SKM_APPLY_MIN_BLOCKS(NW)) k
                 bin_store(tab, a.bins, a.counters, k, st.pay[idx], st.rnk[idx]);
                 my_new++;   // an upper bound of the new keys: the CTA's credit is settled with it, C_DISTINCT comes from the build
             } else {
-                my_new += table_merge(tab, k, st.pay[idx], st.rnk[idx]);
+                bool claimed;
+                table_merge<true>(tab, k, st.pay[idx], st.rnk[idx], &claimed);
+                my_new += claimed;
             }
             st.key[idx] = EMPTY64;
             st.pay[idx] = PAYLOAD_FRESH;

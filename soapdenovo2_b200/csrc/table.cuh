@@ -4,8 +4,9 @@
 //   reference                                       here
 //   P prime-sized sets, one thread per set          ONE power-of-two table in HBM, every thread inserts anywhere
 //   2-bit flag array + 24/40 B kmer_t               32 B (K<=63) / 64 B (K<=127) sector-aligned slots, no flag array
-//   put_kmerset: probe, memset+init | update        128-bit atomicCAS claim of the key, then ONE 128-bit atomicCAS on
-//   (newhash.c:473-528, 74-140)                     {payload, rank}: saturating link/coverage counters + min(first-seen rank)
+//   put_kmerset: probe, memset+init | update        128-bit atomicCAS claim of the key (table_probe), then a 64-bit CAS loop on
+//   (newhash.c:473-528, 74-140)                     payload (saturating link/coverage counters, payload_fold) + a 64-bit atomicMin
+//                                                   on the rank (min first-seen rank, rank_min)
 // The payload word has EXACTLY the reference's kmer_t bit layout (newhash.h:77-102) so that later phases and the
 // parity dump can use it verbatim:
 //   bits  0..23  l_links (4 x 6 bit, index = base code)   bits 24..31  cov (8 bit, saturates at 255)
@@ -228,159 +229,171 @@ PG_D void slot_load(const Slot<NW>* s, Kmer<NW>& k, u64& pay, u64& rank) {
     }
 }
 
-// Find-or-claim the slot of key k.  Returns the slot index; *claimed = true if this call inserted the key.
-template <int NW>
-PG_D u64 table_find_or_claim(const Table<NW>& t, const Kmer<NW>& k, bool* claimed);
-
-template <>
-PG_D u64 table_find_or_claim<2>(const Table<2>& t, const Kmer<2>& k, bool* claimed) {
+// The one linear probe of the global table, from the key's home slot.  CLAIM (find-or-claim): an empty slot is claimed for the key, and
+// *claimed tells whether this call claimed it.  Else (find, in a frozen table): an empty slot ends the probe and the call returns ~0, the
+// key is absent (search_kmerset, newhash.c:277-318).  ENTRY (find-or-claim at K <= 63): each probe reads the whole 32 B sector (ld256),
+// and *entry receives the {payload, rank} that arrived with the key, or {PAYLOAD_FRESH, ~0} (the memset state) after a claim: a hit
+// needs no second read.
+template <bool CLAIM, bool ENTRY = false, int NW>
+PG_D u64 table_probe(const Table<NW>& t, const Kmer<NW>& k, bool* claimed = nullptr, U128* entry = nullptr) {
+    static_assert(!ENTRY || (CLAIM && NW == 2), "a 256-bit key's {payload, rank} is in the next sector");
     u64 idx = table_hash(k) & t.mask;
-    *claimed = false;
+    if (CLAIM) *claimed = false;
     for (;;) {
-        Slot<2>* s = t.slots + idx;
-        U128 cur = ldcg128(s->key);
-        if (cur.a == k.w[0] && cur.b == k.w[1]) return idx;
-        if (cur.a == EMPTY64 && cur.b == EMPTY64) {
-            U128 want{k.w[0], k.w[1]}, empty{EMPTY64, EMPTY64};
-            U128 old = atomicCAS(reinterpret_cast<U128*>(s->key), empty, want);   // ATOMG.E.CAS.128
-            if (old.a == EMPTY64 && old.b == EMPTY64) { *claimed = true; return idx; }
-            if (old.a == k.w[0] && old.b == k.w[1]) return idx;
-        }
-        idx = (idx + 1) & t.mask;
-    }
-}
-
-// 256-bit keys: claim {w0|BUSY, w1} with one 128-bit CAS, publish {w2,w3}, then clear BUSY.  A reader only has to
-// wait when the upper halves match (i.e. it is very likely looking at its own key being published).
-template <>
-PG_D u64 table_find_or_claim<4>(const Table<4>& t, const Kmer<4>& k, bool* claimed) {
-    u64 idx = table_hash(k) & t.mask;
-    *claimed = false;
-    for (;;) {
-        Slot<4>* s = t.slots + idx;
-        U128 hi = ldcg128(&s->key[0]);
-        if (hi.a == EMPTY64 && hi.b == EMPTY64) {
-            U128 want{k.w[0] | BUSY_BIT, k.w[1]}, empty{EMPTY64, EMPTY64};
-            U128 old = atomicCAS(reinterpret_cast<U128*>(&s->key[0]), empty, want);
-            if (old.a == EMPTY64 && old.b == EMPTY64) {
-                stcg128(&s->key[2], U128{k.w[2], k.w[3]});
-                // publish with a release store (orders the lower half before it) instead of __threadfence() + exchange: the fence
-                // compiles to MEMBAR.SC + CCTL.IVALL, paid by every new 256-bit key (a third of the instances at K=127)
-                asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(&s->key[0]), "l"(k.w[0]) : "memory");
-                *claimed = true;
+        Slot<NW>* s = t.slots + idx;
+        if constexpr (NW == 2) {
+            // 128-bit keys: one 128-bit CAS claims the key
+            U128 key, ent;
+            if constexpr (ENTRY) {
+                const U256 v = ld256(s);
+                key = U128{v.a, v.b};
+                ent = U128{v.c, v.d};
+            } else {
+                key = ldcg128(s->key);
+            }
+            if (!CLAIM && key.a == EMPTY64 && key.b == EMPTY64) return ~0ull;
+            if (key.a == k.w[0] && key.b == k.w[1]) {
+                if constexpr (ENTRY) *entry = ent;
                 return idx;
             }
-            hi = old;
-        }
-        if ((hi.a & ~BUSY_BIT) == k.w[0] && hi.b == k.w[1]) {
-            // wait (acquire) until the lower half has been published, then compare it
-            do { hi.a = ldacq64(&s->key[0]); } while (hi.a & BUSY_BIT);
-            U128 lo = ldcg128(&s->key[2]);
-            if (hi.a == k.w[0] && lo.a == k.w[2] && lo.b == k.w[3]) return idx;
+            if (CLAIM && key.a == EMPTY64 && key.b == EMPTY64) {
+                const U128 old = atomicCAS(reinterpret_cast<U128*>(s->key), U128{EMPTY64, EMPTY64}, U128{k.w[0], k.w[1]});   // ATOMG.E.CAS.128
+                if (old.a == EMPTY64 && old.b == EMPTY64) {
+                    *claimed = true;
+                    if (ENTRY) *entry = U128{PAYLOAD_FRESH, EMPTY64};
+                    return idx;
+                }
+                if (old.a == k.w[0] && old.b == k.w[1]) {
+                    if (ENTRY) *entry = ldcg128(&s->payload);
+                    return idx;
+                }
+            }
+        } else {
+            // 256-bit keys: claim {w0|BUSY, w1} with one 128-bit CAS, publish {w2,w3}, then clear BUSY.  A reader only has to wait when
+            // the upper halves match (i.e. it is very likely looking at its own key being published).  The claim in shared memory
+            // (smem_find_or_claim) takes the same steps with one 64-bit CAS on w0.  A frozen table holds no BUSY bit.
+            U128 hi = ldcg128(&s->key[0]);
+            if (hi.a == EMPTY64 && hi.b == EMPTY64) {
+                if (!CLAIM) return ~0ull;
+                const U128 old = atomicCAS(reinterpret_cast<U128*>(&s->key[0]), U128{EMPTY64, EMPTY64}, U128{k.w[0] | BUSY_BIT, k.w[1]});
+                if (old.a == EMPTY64 && old.b == EMPTY64) {
+                    stcg128(&s->key[2], U128{k.w[2], k.w[3]});
+                    // publish with a release store (orders the lower half before it) instead of __threadfence() + exchange: the fence
+                    // compiles to MEMBAR.SC + CCTL.IVALL, paid by every new 256-bit key (a third of the instances at K=127)
+                    asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(&s->key[0]), "l"(k.w[0]) : "memory");
+                    *claimed = true;
+                    return idx;
+                }
+                hi = old;
+            }
+            if ((CLAIM ? hi.a & ~BUSY_BIT : hi.a) == k.w[0] && hi.b == k.w[1]) {
+                // wait (acquire) until the lower half has been published, then compare it
+                if (CLAIM)
+                    do { hi.a = ldacq64(&s->key[0]); } while (hi.a & BUSY_BIT);
+                const U128 lo = ldcg128(&s->key[2]);
+                if (hi.a == k.w[0] && lo.a == k.w[2] && lo.b == k.w[3]) return idx;
+            }
         }
         idx = (idx + 1) & t.mask;
     }
 }
-
-// Read-only lookup (frozen table).  Returns slot index or ~0 when absent (search_kmerset, newhash.c:277-318).
+// Find-or-claim the slot of key k.  Returns the slot index; *claimed = true if this call inserted the key.
 template <int NW>
-PG_D u64 table_find(const Table<NW>& t, const Kmer<NW>& k) {
-    u64 idx = table_hash(k) & t.mask;
+PG_D u64 table_find_or_claim(const Table<NW>& t, const Kmer<NW>& k, bool* claimed) { return table_probe<true>(t, k, claimed); }
+// Read-only lookup (frozen table).  Returns slot index or ~0 when absent.
+template <int NW>
+PG_D u64 table_find(const Table<NW>& t, const Kmer<NW>& k) { return table_probe<false>(t, k); }
+
+// The updates of a slot's {payload, aux} words, in the global table or in a table in shared memory.  EVERY writer of these words
+// (per-instance insert, aggregation, spills, region build, merges) uses the same two 64-bit atomics: atomics of different widths on
+// overlapping words are not guaranteed to be atomic with respect to each other.  Order-independent: the final {payload, rank} is a
+// pure function of the multiset of instances (SURVEY.md A.3).
+// The payload word, whose value was `cur` when read: a 64-bit CAS loop folds `step` into it (payload_apply_n: instances;
+// payload_merge: a partial aggregate).  A step that changes nothing (saturated) is read-only.
+template <class Step>
+PG_D void payload_fold(u64* pay, u64 cur, Step step) {
     for (;;) {
-        const Slot<NW>* s = t.slots + idx;
-        U128 hi = ldcg128(&s->key[0]);
-        if (hi.a == EMPTY64 && hi.b == EMPTY64) return ~0ull;
-        bool m = hi.a == k.w[0] && hi.b == k.w[1];
-        if (NW == 4 && m) {
-            U128 lo = ldcg128(&s->key[2]);
-            m = lo.a == k.w[2] && lo.b == k.w[3];
-        }
-        if (m) return idx;
-        idx = (idx + 1) & t.mask;
+        const u64 nxt = step(cur);
+        if (nxt == cur) break;
+        const u64 old = atomicCAS(pay, cur, nxt);
+        if (old == cur) break;
+        cur = old;
     }
 }
-
-// Apply one k-mer instance: saturating counters through a 64-bit CAS loop on `payload`, first-occurrence rank through an
-// atomicMin on `aux` that is only issued when this instance is an earlier occurrence than the one on record.  EVERY writer of a
-// slot's {payload, aux} words (per-instance insert, aggregated merge, spills) uses these same two 64-bit atomics: atomics of
-// different widths on overlapping words are not guaranteed to be atomic with respect to each other.
-// Order-independent: the final {payload, rank} is a pure function of the multiset of instances (SURVEY.md A.3).
-// c > 1: c identical instances (payload_apply_n).
-template <int NW>
-PG_D void slot_apply(Slot<NW>* s, u64 cur_payload, u64 cur_rank, unsigned left, unsigned right, u64 rank, unsigned c = 1) {
-    for (;;) {
-        u64 nxt = payload_apply_n(cur_payload, left, right, c);
-        if (nxt == cur_payload) break;                       // saturated: read-only
-        u64 old = atomicCAS(&s->payload, cur_payload, nxt);
-        if (old == cur_payload) break;
-        cur_payload = old;
-    }
-    if (rank < cur_rank) atomicMin(&s->aux, rank);
+// The first-occurrence rank: atomicMin, issued only when `earlier` (the rank is below the one read with the payload, where one was read)
+PG_D void rank_min(u64* rnk, u64 rank, bool earlier = true) {
+    if (earlier) atomicMin(rnk, rank);
+}
+// A partial aggregate into an entry whose payload word was `cur` when read
+PG_D void slot_merge(u64* pay, u64* rnk, u64 cur, u64 agg, u64 rank) {
+    payload_fold(pay, cur, [agg](u64 p) { return payload_merge(p, agg); });
+    rank_min(rnk, rank);
 }
 
 // Fused find-or-claim + apply for one k-mer instance (c identical instances).  Returns true if this call inserted the key.
 template <int NW>
-PG_D bool table_insert(const Table<NW>& t, const Kmer<NW>& k, unsigned left, unsigned right, u64 rank, u64* idx_out = nullptr, unsigned c = 1) {
+PG_D bool table_insert(const Table<NW>& t, const Kmer<NW>& k, unsigned left, unsigned right, u64 rank, unsigned c = 1) {
     bool claimed;
-    u64 idx = table_find_or_claim(t, k, &claimed);
-    if (idx_out) *idx_out = idx;
-    Slot<NW>* s = t.slots + idx;
-    U128 cur = claimed ? U128{PAYLOAD_FRESH, EMPTY64} : ldcg128(&s->payload);
-    slot_apply(s, cur.a, cur.b, left, right, rank, c);
-    return claimed;
-}
-// K <= 63: the whole 32 B slot arrives with one sector read per probe (ld256), so a hit needs no second read before the CAS and
-// a fresh claim knows the {payload, rank} it will find (the memset state).
-template <>
-PG_D bool table_insert<2>(const Table<2>& t, const Kmer<2>& k, unsigned left, unsigned right, u64 rank, u64* idx_out, unsigned c) {
-    u64 idx = table_hash(k) & t.mask;
-    bool claimed = false;
     U128 cur;
-    Slot<2>* s;
-    for (;;) {
-        s = t.slots + idx;
-        U256 v = ld256(s);
-        if (v.a == k.w[0] && v.b == k.w[1]) { cur.a = v.c; cur.b = v.d; break; }
-        if (v.a == EMPTY64 && v.b == EMPTY64) {
-            U128 want{k.w[0], k.w[1]}, empty{EMPTY64, EMPTY64};
-            U128 old = atomicCAS(reinterpret_cast<U128*>(s->key), empty, want);
-            if (old.a == EMPTY64 && old.b == EMPTY64) { claimed = true; cur.a = PAYLOAD_FRESH; cur.b = EMPTY64; break; }
-            if (old.a == k.w[0] && old.b == k.w[1]) { cur = ldcg128(&s->payload); break; }
-        }
-        idx = (idx + 1) & t.mask;
-    }
-    if (idx_out) *idx_out = idx;
-    slot_apply(s, cur.a, cur.b, left, right, rank, c);
+    Slot<NW>* s = t.slots + table_probe<true, NW == 2>(t, k, &claimed, &cur);
+    if (NW != 2) cur = claimed ? U128{PAYLOAD_FRESH, EMPTY64} : ldcg128(&s->payload);
+    payload_fold(&s->payload, cur.a, [=](u64 p) { return payload_apply_n(p, left, right, c); });
+    rank_min(&s->aux, rank, rank < cur.b);
     return claimed;
 }
 
-// A partial aggregate into an entry whose payload word was `cur` when read: the 64-bit CAS + atomicMin protocol every writer uses,
-// on the {payload, rank} words of a table slot or of a slot of a region built in shared memory
-PG_D void slot_merge(u64* pay, u64* rnk, u64 cur, u64 agg, u64 rank) {
-    for (;;) {
-        u64 nxt = payload_merge(cur, agg);
-        if (nxt == cur) break;
-        u64 old = atomicCAS(pay, cur, nxt);
-        if (old == cur) break;
-        cur = old;
-    }
-    atomicMin(rnk, rank);
+// One aggregate {agg, rank} of key k into the global table.  Returns the slot index; *claimed = true if this call inserted the key.
+// SOLE (the aggregation's merge mode): a k-mer lives in exactly one bucket and a bucket is aggregated by one CTA at a time, so when this
+// call CLAIMS the slot nobody else can be touching its {payload, aux} words: they are written with one plain 16-byte store (probe load
+// -> claim CAS -> store: two dependent memory round trips per new key).  Else (the region build's remnant list) several entries may
+// hold partials of one key, so a claim merges into the empty slot's {PAYLOAD_FRESH, ~0} like any other writer.  A key that already
+// exists is merged with slot_merge.
+template <bool SOLE, int NW>
+PG_D u64 table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank, bool* claimed) {
+    const u64 idx = table_find_or_claim(t, k, claimed);
+    Slot<NW>* s = t.slots + idx;
+    if (SOLE && *claimed) stcg128(&s->payload, U128{agg, rank});
+    else slot_merge(&s->payload, &s->aux, *claimed ? PAYLOAD_FRESH : ldcg64(&s->payload), agg, rank);
+    return idx;
 }
 
-// One aggregated k-mer -> the global table (merge mode, or a launch after the pass's first).  A k-mer lives in exactly one bucket and a
-// bucket is aggregated by one CTA at a time, so when this call CLAIMS the slot nobody else can be touching its {payload, aux} words:
-// they are written with one plain 16-byte store (probe load -> claim CAS -> store: two dependent memory round trips per new key).  A key
-// that already exists (earlier epoch, or a lane of this bucket spilled the key) is merged with slot_merge.
-template <int NW>
-PG_D bool table_merge(const Table<NW>& t, const Kmer<NW>& k, u64 agg, u64 rank) {
-    bool claimed;
-    u64 idx = table_find_or_claim(t, k, &claimed);
-    Slot<NW>* s = t.slots + idx;
-    if (claimed) {
-        stcg128(&s->payload, U128{agg, rank});
-        return true;
+// Find or claim key k in a table in SHARED memory by linear probing from slot `idx` (left at the key's slot).  Key word w of slot j is
+// key[j * slot_stride + w * word_stride].  WRAP: the probe wraps around at slot n and gives up after n probes; else it gives up at
+// slot n.  Claim: CAS(w0, EMPTY -> w0|BUSY), write the other key words, `fill(j)` (what else the claimer writes before it publishes),
+// fence, store w0.  A thread that meets a BUSY w0 whose other bits match waits for the publication (independent thread scheduling: the
+// claimer makes progress even inside the same warp).  `room()` is read before each claim: false makes the call give up (a claim limit).
+// Returns false when the call gave up; else it has called done(j, claimed) with the key's slot j.
+template <int NW, bool WRAP, class Room, class Fill, class Done>
+PG_D bool smem_find_or_claim(u64* key, u32 slot_stride, u32 word_stride, u32 n, const Kmer<NW>& k, u32& idx, Room room, Fill fill, Done done) {
+    for (u32 probe = 0; WRAP ? probe < n : idx < n; probe++) {
+        u64* const sl = key + (u64)idx * slot_stride;
+        volatile u64* const ks = sl;
+        u64 k0 = ks[0];
+        if (k0 == EMPTY64) {
+            if (!room()) return false;
+            k0 = atomicCAS(sl, EMPTY64, k.w[0] | BUSY_BIT);
+            if (k0 == EMPTY64) {
+#pragma unroll
+                for (int w = 1; w < NW; w++) ks[w * word_stride] = k.w[w];
+                fill(idx);
+                __threadfence_block();
+                ks[0] = k.w[0];
+                done(idx, true);
+                return true;
+            }
+        }
+        if ((k0 & ~BUSY_BIT) == k.w[0]) {
+            while (k0 & BUSY_BIT) k0 = ks[0];
+            bool same = true;
+#pragma unroll
+            for (int w = 1; w < NW; w++) same = same && ks[w * word_stride] == k.w[w];
+            if (same) {
+                done(idx, false);
+                return true;
+            }
+        }
+        idx = WRAP && idx + 1 == n ? 0u : idx + 1;
     }
-    slot_merge(&s->payload, &s->aux, ldcg64(&s->payload), agg, rank);
     return false;
 }
 

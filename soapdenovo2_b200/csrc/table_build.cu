@@ -28,43 +28,6 @@ struct TableBuildArgs {
     u64 spill_cap;
 };
 
-// One entry of a bin into the region in shared memory (RS slots in table format), by linear probing WITHOUT wrap-around from the key's
-// home slot.  Claim: CAS(key0, EMPTY -> w0|BUSY), the other words and {payload, rank}, fence, publish w0 (a new key: ++n_new); a match
-// merges its partial.  Returns false when every probe ran off the region's end: a carry.
-template <int NW>
-__device__ __forceinline__ bool region_place(u64* s_reg, u32 RS, const Kmer<NW>& k, u64 pay, u64 rank, unsigned& n_new) {
-    constexpr int SW = (int)sizeof(Slot<NW>) / 8;   // words per slot
-    for (u32 j = (u32)(table_hash(k) & (RS - 1)); j < RS; j++) {
-        u64* const sl = s_reg + (u64)j * SW;
-        volatile u64* const ks = sl;
-        u64 k0 = ks[0];
-        if (k0 == EMPTY64) {
-            k0 = atomicCAS((unsigned long long*)sl, EMPTY64, k.w[0] | BUSY_BIT);
-            if (k0 == EMPTY64) {
-#pragma unroll
-                for (int w = 1; w < NW; w++) ks[w] = k.w[w];
-                ks[NW] = pay;
-                ks[NW + 1] = rank;
-                __threadfence_block();
-                ks[0] = k.w[0];
-                n_new++;
-                return true;
-            }
-        }
-        if ((k0 & ~BUSY_BIT) == k.w[0]) {
-            while (k0 & BUSY_BIT) k0 = ks[0];
-            bool same = true;
-#pragma unroll
-            for (int w = 1; w < NW; w++) same = same && ks[w] == k.w[w];
-            if (same) {
-                slot_merge(sl + NW, sl + NW + 1, ks[NW], pay, rank);
-                return true;
-            }
-        }
-    }
-    return false;
-}
-
 template <int NW>
 __global__ void __launch_bounds__(TB_THREADS) k_table_build(Table<NW> tab, TableBuildArgs a) {
     constexpr int SW = (int)sizeof(Slot<NW>) / 8;   // words per slot
@@ -89,7 +52,21 @@ __global__ void __launch_bounds__(TB_THREADS) k_table_build(Table<NW> tab, Table
             Kmer<NW> k;
             u64 pay, rank;
             slot_load(g + i, k, pay, rank);
-            if (region_place(s_reg, RS, k, pay, rank, my_new)) continue;
+            // into the region by linear probing WITHOUT wrap-around from the key's home slot: a claim writes {payload, rank} before it
+            // publishes the key (a new key), a match merges its partial; a carry when every probe runs off the region's end
+            u32 j = (u32)(table_hash(k) & (RS - 1));
+            if (smem_find_or_claim<NW, false>(s_reg, SW, 1, RS, k, j, [] { return true; },
+                                              [&](u32 j) {
+                                                  volatile u64* const ks = s_reg + (u64)j * SW;
+                                                  ks[NW] = pay;
+                                                  ks[NW + 1] = rank;
+                                              },
+                                              [&](u32 j, bool claimed) {
+                                                  u64* const sl = s_reg + (u64)j * SW;
+                                                  if (claimed) my_new++;
+                                                  else slot_merge(sl + NW, sl + NW + 1, ((volatile u64*)sl)[NW], pay, rank);
+                                              }))
+                continue;
             const u64 c = atomicAdd(&a.counters[C_CARRY], 1ull);   // a carry
             if (c < a.bins.remnant_cap) slot_store(reinterpret_cast<Slot<NW>*>(a.bins.remnant) + c, k, pay, rank);
         }
@@ -123,9 +100,7 @@ __global__ void __launch_bounds__(256) k_merge_remnants(Table<NW> tab, TableBuil
         u64 pay, rank;
         slot_load(list + i, k, pay, rank);
         bool claimed;
-        const u64 idx = table_find_or_claim(tab, k, &claimed);
-        Slot<NW>* const s = tab.slots + idx;
-        slot_merge(&s->payload, &s->aux, claimed ? PAYLOAD_FRESH : ldcg64(&s->payload), pay, rank);
+        const u64 idx = table_merge<false>(tab, k, pay, rank, &claimed);
         if (claimed) {
             my_new++;
             const u64 sn = atomicAdd((unsigned long long*)&a.counters[C_SPILLKEYS], 1ull);
