@@ -59,6 +59,22 @@ __device__ __forceinline__ void mbar_wait(u64* bar, unsigned parity) {
                  "r"(parity)
                  : "memory");
 }
+// an arrival that expects no bytes (a stage with nothing to copy)
+__device__ __forceinline__ void mbar_arrive(u64* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// The other direction: a bulk copy from shared to global memory (SASS UBLKCP.G.S), tracked in the issuing thread's bulk async-groups.
+// Generic-proxy writes of the source must be ordered before it by fence.proxy.async.shared::cta in every writing thread, then a barrier.
+__device__ __forceinline__ void tma_bulk_s2g(void* dst, const void* src, unsigned bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// until at most N of this thread's committed groups still read their source (the older ones' shared memory may be written again)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// until every committed group has completed (its global writes are done)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 #endif
 
 }   // namespace pgb

@@ -1,23 +1,27 @@
 // table_build.cu -- aggregated pass 1, the region build of the k-mer table.
 // The table of a launch into an empty table is a pure function of its aggregates, and its slot positions are private to the engine (any
-// valid linear-probing placement will do): so it is built like a partitioned hash build.  One CTA per region (grid-stride): fill the
-// region in shared memory with EMPTY, read the bin's entries (the region's own table memory, written by k_skm_apply<NW, true>), find or
-// claim each key by linear probing WITHOUT wrap-around and merge its partials, sweep every occupied slot, write the region out whole,
-// empty slots included.  Every partial of a key lands in the same bin, and slots never empty again, so a key is either entirely in the
-// region -- final, and swept here -- or all its probes run off the region's end: a carry, appended to the remnant list and merged by
-// k_merge_remnants once every region is written.  Regions of 64 KB let 3 CTAs share an SM (one region's fill, read, probe and
-// write-back overlap another's); a bin holds 2048 (K <= 63) or 1024 slots' worth of entries, twice the expected fill at 0.85 load.
-// The end-of-pass sweeps -- delow, linear flag, coverage histogram (thread_delow / thread_mark / freqStat, prlHashReads.c:953-1132) --
-// are applied to every entry as its region is written.
+// valid linear-probing placement will do): so it is built like a partitioned hash build.  Each region (RS slots) is made in shared
+// memory: fill with EMPTY, find or claim each entry of the bin (the region's own table memory, written by k_skm_apply<NW, true>) by
+// linear probing WITHOUT wrap-around and merge its partials, sweep every occupied slot, write the region out whole, empty slots
+// included.  Every partial of a key lands in the same bin, and slots never empty again, so a key is either entirely in the region --
+// final, and swept here -- or all its probes run off the region's end: a carry, appended to the remnant list and merged by
+// k_merge_remnants once every region is written.
+// What bounds the build is the memory traffic each SM keeps in flight, not issue: so a CTA is a pipeline over its regions (grid-stride),
+// with every byte of a bin and of a region moved by bulk copies.  While it builds region i, the bin of region i+1 arrives in the other
+// stage (one cp.async.bulk, complete on that stage's mbarrier) and region i-1 leaves from the other region buffer (one bulk store):
+// two region buffers of RS slots and two stages of 256 entries.  A bin holds at most RS entries (bin_store); one larger than its stage
+// arrives in pieces.  The end-of-pass sweeps -- delow, linear flag, coverage histogram (thread_delow / thread_mark / freqStat,
+// prlHashReads.c:953-1132) -- are applied to every entry as its region is written.
 #include "engine_impl.cuh"
 #include "table_build.cuh"
+#include "chop.cuh"
 
 namespace pgb {
 
 constexpr int TB_THREADS = 256;   // one coverage-histogram bin per thread (SweepTally)
-constexpr int TB_REGION_BYTES = 64 * 1024;
-template <int NW>
-constexpr int tb_region_log2() { return __builtin_ctz(TB_REGION_BYTES / (int)sizeof(Slot<NW>)); }
+constexpr int TB_REGION_LOG2 = 9;           // 512 slots: 16 KB regions at K <= 63 (4 CTAs per SM), 32 KB above (2 CTAs per SM)
+constexpr u32 TB_STAGE_SLOTS = 256;         // entries per stage; a bin of more arrives in pieces
+__host__ __device__ constexpr u32 tb_stage_slots(u32 region_slots) { return region_slots < TB_STAGE_SLOTS ? region_slots : TB_STAGE_SLOTS; }
 
 struct TableBuildArgs {
     BinArgs bins;
@@ -28,57 +32,112 @@ struct TableBuildArgs {
     u64 spill_cap;
 };
 
+// Dynamic shared memory: region buffers 0 and 1 (RS slots each), then stages 0 and 1 (SE slots each).  Region i of the CTA uses buffer
+// and stage i & 1.
 template <int NW>
 __global__ void __launch_bounds__(TB_THREADS) k_table_build(Table<NW> tab, TableBuildArgs a) {
     constexpr int SW = (int)sizeof(Slot<NW>) / 8;   // words per slot
-    extern __shared__ __align__(16) u64 s_reg[];    // [RS] slots in table format
+    extern __shared__ __align__(128) u64 s_buf[];
     __shared__ SweepTally s_sw;
+    __shared__ u64 s_bar[2];   // stage s is full
+    __shared__ u32 s_n[2];     // entries in the bin that stage s takes
     __shared__ unsigned s_new;
     const int tid = threadIdx.x;
-    const u32 RS = 1u << a.bins.region_log2;
+    const u32 RS = 1u << a.bins.region_log2, SE = tb_stage_slots(RS);
+    const u32 RW = RS * SW;   // words per region buffer
     const u64 n_regions = (tab.mask + 1) >> a.bins.region_log2;
     // a bin overflow leaves partials of some keys on the remnant list, merged after the build: then nothing may be swept here
     const bool sweep = a.sweep && ldcg64(&a.counters[C_BIN_OVF]) == 0;
-    s_sw.clear();
-    if (tid == 0) s_new = 0;
-    unsigned lin = 0, rem = 0, my_new = 0;
-    for (u64 r = blockIdx.x; r < n_regions; r += gridDim.x) {
-        __syncthreads();   // the previous region is written out
-        for (u32 i = tid; i < RS * SW / 2; i += TB_THREADS) reinterpret_cast<uint4*>(s_reg)[i] = make_uint4(~0u, ~0u, ~0u, ~0u);
-        __syncthreads();
-        Slot<NW>* const g = tab.slots + (r << a.bins.region_log2);
-        const u32 n = min(a.bins.cursor[r], RS);
-        for (u32 i = tid; i < n; i += TB_THREADS) {
-            Kmer<NW> k;
-            u64 pay, rank;
-            slot_load(g + i, k, pay, rank);
-            // into the region by linear probing WITHOUT wrap-around from the key's home slot: a claim writes {payload, rank} before it
-            // publishes the key (a new key), a match merges its partial; a carry when every probe runs off the region's end
-            u32 j = (u32)(table_hash(k) & (RS - 1));
-            if (smem_find_or_claim<NW, false>(s_reg, SW, 1, RS, k, j, [] { return true; },
-                                              [&](u32 j) {
-                                                  volatile u64* const ks = s_reg + (u64)j * SW;
-                                                  ks[NW] = pay;
-                                                  ks[NW + 1] = rank;
-                                              },
-                                              [&](u32 j, bool claimed) {
-                                                  u64* const sl = s_reg + (u64)j * SW;
-                                                  if (claimed) my_new++;
-                                                  else slot_merge(sl + NW, sl + NW + 1, ((volatile u64*)sl)[NW], pay, rank);
-                                              }))
-                continue;
-            const u64 c = atomicAdd(&a.counters[C_CARRY], 1ull);   // a carry
-            if (c < a.bins.remnant_cap) slot_store(reinterpret_cast<Slot<NW>*>(a.bins.remnant) + c, k, pay, rank);
+    // one thread moves the bins in: m entries from src into stage s, or an arrival without bytes when there are none
+    auto piece_in = [&](const Slot<NW>* src, u32 m, int s) {
+        if (m) {
+            mbar_expect_tx(&s_bar[s], m * (u32)sizeof(Slot<NW>));
+            tma_bulk_g2s(s_buf + 2 * RW + s * SE * SW, src, m * (u32)sizeof(Slot<NW>), &s_bar[s]);
+        } else {
+            mbar_arrive(&s_bar[s]);
         }
-        __syncthreads();   // every entry of the bin is read and placed: its table memory may be overwritten
+    };
+    auto bin_in = [&](u64 r, u32 cursor, int s) {
+        const u32 n = min(cursor, RS);
+        s_n[s] = n;
+        piece_in(tab.slots + (r << a.bins.region_log2), min(n, SE), s);
+    };
+    s_sw.clear();
+    u32 c_next = 0;   // thread 0: the cursor of the bin after the one in flight, read one region ahead of its use
+    if (tid == 0) {
+        s_new = 0;
+        mbar_init(&s_bar[0], 1);
+        mbar_init(&s_bar[1], 1);
+        bin_in(blockIdx.x, a.bins.cursor[blockIdx.x], 0);   // (the grid has no more CTAs than regions)
+        if (blockIdx.x + gridDim.x < n_regions) c_next = a.bins.cursor[blockIdx.x + gridDim.x];
+    }
+    unsigned lin = 0, rem = 0, my_new = 0;
+    u32 it = 0, phase = 0;   // bit s: the parity of the next wait on stage s
+    for (u64 r = blockIdx.x; r < n_regions; r += gridDim.x, it++) {
+        const int b = it & 1;
+        u64* const reg = s_buf + b * RW;
+        const u64* const stage = s_buf + 2 * RW + b * SE * SW;
+        Slot<NW>* const g = tab.slots + (r << a.bins.region_log2);
+        // the other stage was read by region it-1 (fence.proxy.async and the barrier at its end): the next bin goes there
+        if (tid == 0 && r + gridDim.x < n_regions) {
+            bin_in(r + gridDim.x, c_next, b ^ 1);
+            if (r + 2ull * gridDim.x < n_regions) c_next = a.bins.cursor[r + 2ull * gridDim.x];
+        }
+        // this buffer's store (region it-2) has finished reading it: waited for before region it-1's store was issued
+        for (u32 i = tid; i < RW / 2; i += TB_THREADS) reinterpret_cast<uint4*>(reg)[i] = make_uint4(~0u, ~0u, ~0u, ~0u);
+        __syncthreads();   // the region is EMPTY; s_n[b] is written
+        const u32 n = s_n[b];
+        for (u32 p0 = 0;;) {
+            mbar_wait(&s_bar[b], (phase >> b) & 1u);
+            phase ^= 1u << b;
+            const u32 m = min(n - p0, SE);
+            for (u32 i = tid; i < m; i += TB_THREADS) {
+                const u64* const e = stage + (u64)i * SW;
+                Kmer<NW> k;
+#pragma unroll
+                for (int w = 0; w < NW; w++) k.w[w] = e[w];
+                const u64 pay = e[NW], rank = e[NW + 1];
+                // into the region by linear probing WITHOUT wrap-around from the key's home slot: a claim writes {payload, rank} before it
+                // publishes the key (a new key), a match merges its partial; a carry when every probe runs off the region's end
+                u32 j = (u32)(table_hash(k) & (RS - 1));
+                if (smem_find_or_claim<NW, false>(reg, SW, 1, RS, k, j, [] { return true; },
+                                                  [&](u32 j) {
+                                                      volatile u64* const ks = reg + (u64)j * SW;
+                                                      ks[NW] = pay;
+                                                      ks[NW + 1] = rank;
+                                                  },
+                                                  [&](u32 j, bool claimed) {
+                                                      u64* const sl = reg + (u64)j * SW;
+                                                      if (claimed) my_new++;
+                                                      else slot_merge(sl + NW, sl + NW + 1, ((volatile u64*)sl)[NW], pay, rank);
+                                                  }))
+                    continue;
+                const u64 c = atomicAdd(&a.counters[C_CARRY], 1ull);   // a carry
+                if (c < a.bins.remnant_cap) slot_store(reinterpret_cast<Slot<NW>*>(a.bins.remnant) + c, k, pay, rank);
+            }
+            p0 += SE;
+            if (p0 >= n) break;
+            // a bin larger than the stage: its next piece into the same stage, once every thread has read this one
+            fence_proxy_async_smem();
+            __syncthreads();
+            if (tid == 0) piece_in(g + p0, min(n - p0, SE), b);
+        }
+        __syncthreads();   // every entry is placed
         if (sweep)
             for (u32 j = tid; j < RS; j += TB_THREADS) {
-                u64* const sl = s_reg + (u64)j * SW;
+                u64* const sl = reg + (u64)j * SW;
                 if (!(sl[0] == EMPTY64 && sl[1] == EMPTY64)) sl[NW] = sweep_payload(sl[NW], a.D, rem, lin, s_sw.hist);
             }
+        // this thread's writes of the region and reads of the stage come before the bulk copies that read or overwrite them
+        fence_proxy_async_smem();
+        if (tid == 0) bulk_wait_read<0>();   // region it-1's store no longer reads the other buffer, which region it+1 fills
         __syncthreads();
-        for (u32 i = tid; i < RS * SW / 2; i += TB_THREADS) stcg128(reinterpret_cast<U128*>(g) + i, reinterpret_cast<const U128*>(s_reg)[i]);
+        if (tid == 0) {
+            tma_bulk_s2g(g, reg, RS * (u32)sizeof(Slot<NW>));
+            bulk_commit();
+        }
     }
+    if (tid == 0) bulk_wait_all();   // the region stores read shared memory until they complete, and the CTA's table is written
     if (my_new) atomicAdd(&s_new, my_new);
     s_sw.flush(lin, rem, a.hist, &a.counters[C_LINEAR], &a.counters[C_REMOVED]);   // (synchronises the CTA first)
     if (tid == 0 && s_new) atomicAdd(&a.counters[C_DISTINCT], (u64)s_new);
@@ -121,10 +180,10 @@ BinArgs EngineT<NW>::bin_args() const {
 // Before a region-mode aggregation launch: the region size, empty bins, room for the remnant list, and cleared build counters
 template <int NW>
 void EngineT<NW>::table_build_prepare() {
-    int rl = tb_region_log2<NW>();
+    int rl = TB_REGION_LOG2;
     if (const char* e = getenv("PGB200_TABLE_REGION")) {   // slots per region (a power of two; tests use tiny regions for carries)
         const u64 v = strtoull(e, nullptr, 0);
-        if (v < 1 || (v & (v - 1)) || v > (1ull << rl)) throw std::runtime_error("pgb200: PGB200_TABLE_REGION must be a power of two up to the 64 KB region");
+        if (v < 1 || (v & (v - 1)) || v > (1ull << rl)) throw std::runtime_error("pgb200: PGB200_TABLE_REGION must be a power of two up to the default region size");
         rl = __builtin_ctzll(v);
     }
     while ((1ull << rl) > cap_) rl--;
@@ -153,8 +212,8 @@ void EngineT<NW>::table_build_launch() {
     b.counters = d_cnt_;
     b.spill_list = spill_list_.template as<u64>();
     b.spill_cap = SPILL_CAP;
-    const size_t smem = sizeof(Slot<NW>) << region_log2_;
-    PG_CUDA(cudaFuncSetAttribute(k_table_build<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, TB_REGION_BYTES));
+    const size_t smem = 2 * sizeof(Slot<NW>) * ((1ull << region_log2_) + tb_stage_slots(1u << region_log2_));   // two region buffers, two stages
+    PG_CUDA(cudaFuncSetAttribute(k_table_build<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
     PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_table_build<NW>, TB_THREADS, smem));
     if (per_sm < 1) per_sm = 1;
