@@ -59,15 +59,6 @@ __global__ void __launch_bounds__(256) k_nl_count(const uint4* __restrict__ text
     }
 }
 
-struct TileCntIn {
-    const u32* a;
-    __device__ u64 operator()(u64 i) const { return a[i]; }
-};
-struct TileBaseOut {
-    u32* a;
-    __device__ void operator()(u64 i, u64 prefix, u64) const { a[i] = (u32)prefix; }
-};
-
 // newline number g (0-based) at byte `pos`: it ends line g and line g+1 starts at pos+1.  Records are lpr = 1 << lshift lines long:
 // line 0 of a record is its header, line 1 its sequence, FASTQ line 2 the '+' separator.
 struct LineIndexCtx {
@@ -321,7 +312,7 @@ DecodeLines decode_lines(const unsigned char* d_text, size_t nbytes, int fastq, 
     const unsigned nl_blocks = (unsigned)std::min<u64>((n_tiles + 7) / 8, (u64)n_sm * 16);
     k_nl_count<<<nl_blocks, 256, 0, sd>>>(t16, (u64)nbytes, n_tiles, tile_cnt);
     PG_CUDA(cudaGetLastError());
-    device_scan(TileCntIn{tile_cnt}, TileBaseOut{tile_base}, n_tiles, scan_tmp, d_cnt + C_MISC0, sd);
+    device_scan(ScanU32In{tile_cnt}, ScanU32Out{tile_base}, n_tiles, scan_tmp, d_cnt + C_MISC0, sd);
     unsigned char* h_last = reinterpret_cast<unsigned char*>(h_cnt + C_COUNT);
     PG_CUDA(cudaMemcpyAsync(h_last, d_text + nbytes - 1, 1, cudaMemcpyDeviceToHost, sd));
     PG_CUDA(cudaMemcpyAsync(h_cnt, d_cnt, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, sd));

@@ -14,9 +14,11 @@
 //   edge id   := 1 + exclusive prefix over emitted starts of (1 + bal_edge)      (edge_c += bal_edge reserves the twin)
 //   text      := prefix sum of per-edge text lengths, then every edge writes its own record
 // Interior nodes get {edgeId overlaid on l_links|cov, twin, inEdge} exactly like the reference's union (newhash.h:83-102).
+// The walk is walk.cuh's, shared with tip clipping; a start's (side, base) is its link there, and rev(start) the walk's `rev`.
 #include "engine_impl.cuh"
 #include "scan.cuh"
 #include "patch.cuh"
+#include "walk.cuh"
 #include <algorithm>
 
 namespace pgb {
@@ -30,50 +32,6 @@ struct EdgeRec {
     u32 status;   // 0 unknown, 1 emitted, 2 suppressed
 };
 
-template <int NW>
-struct EdgeEnd {
-    u64 slot;
-    int sm;
-    Kmer<NW> to, second_last, frm;
-    u32 length;
-    int err;
-};
-
-template <int NW>
-__device__ __forceinline__ void canon2(const Kmer<NW>& w, const KParams<NW>& kp, Kmer<NW>& word, Kmer<NW>& bal, int& sm) {
-    Kmer<NW> b = krc_n(w, kp.K);
-    if (kless(b, w)) { word = b; bal = w; sm = 0; } else { word = w; bal = b; sm = 1; }
-}
-
-// walk the unipath that leaves node `e` through (side, ch); visit.internal(i, slot, sm, ori, payload) for every linear node,
-// i = 1.. ; the terminal node is node number end->length.
-template <int NW, class V>
-__device__ void edge_walk(const Table<NW>& tab, const KParams<NW>& kp, u64 e_slot, int side, unsigned ch, V& visit, EdgeEnd<NW>* end) {
-    Kmer<NW> seq = slot_key(tab.slots + e_slot);
-    Kmer<NW> frm = side == 0 ? seq : krc_n(seq, kp.K);
-    unsigned nextch = side == 0 ? ch : (ch ^ 2u);
-    end->frm = frm; end->err = 0;
-    Kmer<NW> prev = frm, cw, cb;
-    int sm;
-    canon2(knext(frm, nextch, kp), kp, cw, cb, sm);
-    u32 length = 0;
-    for (;;) {
-        u64 os = table_find(tab, cw);
-        if (os == ~0ull) { end->err = 1; end->length = length; return; }
-        u64 po = tab.slots[os].payload;
-        Kmer<NW> ori = sm ? cw : cb;
-        length++;
-        if (!(po & PL_LINEAR)) {
-            end->slot = os; end->sm = sm; end->to = ori; end->second_last = prev; end->length = length;
-            return;
-        }
-        visit.internal(length, os, sm, ori, po);
-        prev = ori;
-        unsigned nc = sm ? (unsigned)pl_first_r(po) : ((unsigned)pl_first_l(po) ^ 2u);
-        canon2(knext(ori, nc, kp), kp, cw, cb, sm);
-    }
-}
-
 // ---------------------------------------------------------------- formatting helpers
 __device__ __forceinline__ int dec_len(u64 v) { int n = 1; while (v >= 10) { v /= 10; n++; } return n; }
 __device__ __forceinline__ int hex_len(u64 v) { return v ? (64 - __clzll((long long)v) + 3) / 4 : 1; }
@@ -83,12 +41,12 @@ __device__ __forceinline__ char* put_str(char* p, const char* s) { while (*s) *p
 template <int NW>
 __device__ int kmer_hex_len(const Kmer<NW>& k, int out_words) {   // "%llx %llx[ %llx %llx]"
     int n = out_words - 1;
-    for (int w = 0; w < out_words; w++) { int src = w - (out_words - NW); n += hex_len(src >= 0 ? k.w[src] : 0ull); }
+    for (int w = 0; w < out_words; w++) n += hex_len(kout_word(k, w, out_words));
     return n;
 }
 template <int NW>
 __device__ char* put_kmer_hex(char* p, const Kmer<NW>& k, int out_words) {
-    for (int w = 0; w < out_words; w++) { int src = w - (out_words - NW); if (w) *p++ = ' '; p = put_hex(p, src >= 0 ? k.w[src] : 0ull); }
+    for (int w = 0; w < out_words; w++) { if (w) *p++ = ' '; p = put_hex(p, kout_word(k, w, out_words)); }
     return p;
 }
 __device__ __forceinline__ u32 edge_cvg(u64 symbol, u32 length) {   // node2edge.c:585-592 (integer division first)
@@ -131,7 +89,10 @@ __device__ __forceinline__ u64 bsearch_u64(const u64* a, u64 n, u64 key) {   // 
 struct SymbolVisit {
     u64 symbol;
     template <int NW>
-    __device__ void internal(u32, u64, int, const Kmer<NW>&, u64 po) { symbol += pl_l(po, 0) + pl_l(po, 1) + pl_l(po, 2) + pl_l(po, 3); }
+    __device__ int operator()(u32, u64, int, const Kmer<NW>&, u64 po) {
+        symbol += pl_l(po, 0) + pl_l(po, 1) + pl_l(po, 2) + pl_l(po, 3);
+        return WALK_GO;
+    }
 };
 
 template <int NW>
@@ -139,15 +100,12 @@ __global__ void __launch_bounds__(128) k_edge_walk(Table<NW> tab, KParams<NW> kp
     for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < S; j += (u64)gridDim.x * blockDim.x) {
         u64 sid = starts[j];
         SymbolVisit sv{0};
-        EdgeEnd<NW> end;
-        edge_walk(tab, kp, order[sid >> 3], (int)((sid >> 2) & 1), (unsigned)(sid & 3), sv, &end);
+        WalkEnd<NW> end = unipath_walk(tab, kp, order[sid >> 3], (unsigned)(sid & 7), sv);
         EdgeRec r;
         r.status = 0; r.symbol = sv.symbol; r.length = end.length; r.rev_id = EMPTY64; r.hdr_len = 0; r.text_len = 0;
-        if (end.err) { atomicAdd(err, 1ull); rec[j] = r; continue; }
+        if (end.status != WALK_REACHED) { atomicAdd(err, 1ull); rec[j] = r; continue; }
         const Slot<NW>* T = tab.slots + end.slot;
-        unsigned c = kfirst(end.second_last, kp);
-        u64 rid = T->aux * 8 + (end.sm ? 4u + c : (c ^ 2u));      // dislink2prevUncertain(last, firstCh(second_last), last.sm)
-        if (!(T->payload & PL_DELETED)) r.rev_id = rid;
+        if (!(T->payload & PL_DELETED)) r.rev_id = T->aux * 8 + end.rev;   // the start at the far end that walks this path back
         u32 cvg = edge_cvg(sv.symbol, end.length);
         // ">length %d,%llx %llx,%llx %llx,cvg %d, %d\n"
         r.hdr_len = 8 + dec_len(end.length) + 1 + kmer_hex_len(end.frm, out_words) + 1 + kmer_hex_len(end.to, out_words) + 1 + 4 + dec_len(cvg) + 2 + 1 + 1;
@@ -199,13 +157,6 @@ struct EmNoRevIn {   // emitted starts whose far end is a deleted node (nothing 
     const EdgeRec* rec;
     __device__ u64 operator()(u64 j) const { return rec[j].status == 1 && rec[j].rev_id == EMPTY64; }
 };
-struct PrefixOut {
-    u64* out;
-    __device__ void operator()(u64 j, u64 prefix, u64) const { out[j] = prefix; }
-};
-struct NullOut {
-    __device__ void operator()(u64, u64, u64) const {}
-};
 
 template <int NW>
 struct EmitVisit {
@@ -217,15 +168,16 @@ struct EmitVisit {
         seq[c + c / 100] = "ACTG"[code];
         if (i % 100 == 0) seq[c + c / 100 + 1] = '\n';
     }
-    __device__ void internal(u32 i, u64 slot, int sm, const Kmer<NW>& ori, u64 po) {
+    __device__ int operator()(u32 i, u64 slot, int sm, const Kmer<NW>& ori, u64 po) {
         put_base(i, klast(ori));
         // a node met twice inside one path keeps the values of its FIRST occurrence (the reference assigns back to front)
-        if (pl_inedge(po)) return;
+        if (pl_inedge(po)) return WALK_GO;
         // The reference overlays edgeId on l_links|cov (union, newhash.h:83-88).  Here the id goes to `aux` (the iteration
         // index is no longer needed for a linear node) so that the link fields stay intact while other walks still read them.
         u64 twin = sm ? (u64)(bal + 1) : (u64)(1 - bal);
         slots[slot].aux = sm ? eid : eid + bal;
         slots[slot].payload = (po & ~(3ull << PL_TWIN_SHIFT)) | (twin << PL_TWIN_SHIFT) | (1ull << PL_INEDGE_SHIFT);
+        return WALK_GO;
     }
 };
 
@@ -241,12 +193,9 @@ __global__ void __launch_bounds__(128) k_edge_emit(Table<NW> tab, KParams<NW> kp
         u32 eid = (u32)(id_prefix[j] + 1);
         char* base = text + text_prefix[j];
         EmitVisit<NW> ev{base + r.hdr_len, tab.slots, eid, bal};
-        EdgeEnd<NW> end;
         u64 e_slot = order[sid >> 3];
-        int side = (int)((sid >> 2) & 1);
-        unsigned ch = (unsigned)(sid & 3);
-        edge_walk(tab, kp, e_slot, side, ch, ev, &end);
-        if (end.err || end.length != r.length) { atomicAdd(err, 1ull); continue; }
+        WalkEnd<NW> end = unipath_walk(tab, kp, e_slot, (unsigned)(sid & 7), ev);
+        if (end.status != WALK_REACHED || end.length != r.length) { atomicAdd(err, 1ull); continue; }
         ev.put_base(end.length, klast(end.to));
         if (end.length % 100 != 0) { u32 c = end.length - 1; ev.seq[c + c / 100 + 1] = '\n'; }
         // header
@@ -258,11 +207,8 @@ __global__ void __launch_bounds__(128) k_edge_emit(Table<NW> tab, KParams<NW> kp
         p = put_dec(p, bal); *p++ = '\n';
         if ((u32)(p - base) != r.hdr_len) atomicAdd(err, 1ull);
         // unlink both ends (dislink2nextUncertain(first) / dislink2prevUncertain(last)); other edges touch the same words
-        u64 m0 = side == 0 ? ~(63ull << (PL_R_SHIFT + 6 * ch)) : ~(63ull << (6 * ch));
-        atomicAnd(&tab.slots[e_slot].payload, m0);
-        unsigned c = kfirst(end.second_last, kp);
-        u64 m1 = end.sm ? ~(63ull << (6 * c)) : ~(63ull << (PL_R_SHIFT + 6 * (c ^ 2u)));
-        atomicAnd(&tab.slots[end.slot].payload, m1);
+        atomicAnd(&tab.slots[e_slot].payload, ~(63ull << link_shift((unsigned)(sid & 7))));
+        atomicAnd(&tab.slots[end.slot].payload, ~(63ull << link_shift(end.rev)));
         if (end.length == 1) {   // (K+1)-mer patch entry, node2edge.c:481-541
             Kmer<NW> wp = kshl2(end.frm);
             wp.w[NW - 1] |= klast(end.to);
@@ -277,7 +223,6 @@ template <int NW>
 void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
     if (!order_buf_.p) throw std::runtime_error("pgb200: build_edges before build_layout");
     const u64 N = n_nodes_;
-    const int out_words = prm_.flavour127 ? 4 : 2;
     u64* order = order_buf_.template as<u64>();
     DevBuf scratch, startsb, recb, claimb, idb, txb, errb, textb;
     scratch.alloc(scan_scratch_elems(N) * sizeof(u64));
@@ -285,16 +230,16 @@ void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
     PG_CUDA(cudaMemsetAsync(errb.p, 0, 2 * sizeof(u64), st_));
     u64* err = errb.template as<u64>();
     // starts
-    device_scan(StartIn<NW>{tab_.slots, order}, NullOut{}, N, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
+    device_scan_total(StartIn<NW>{tab_.slots, order}, N, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
     read_counters();
     const u64 S = h_cnt_[C_MISC0];
     startsb.alloc((S + 1) * sizeof(u64));
     u64* starts = startsb.template as<u64>();
-    device_scan(StartIn<NW>{tab_.slots, order}, StartOut<NW>{tab_.slots, order, starts}, N, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
+    device_scan_finish(StartIn<NW>{tab_.slots, order}, StartOut<NW>{tab_.slots, order, starts}, N, scratch.template as<u64>(), st_);
     recb.alloc((S + 1) * sizeof(EdgeRec));
     EdgeRec* rec = recb.template as<EdgeRec>();
     unsigned blocks = (unsigned)std::min<u64>((S + 127) / 128 + 1, (u64)n_sm_ * 16);
-    k_edge_walk<NW><<<blocks, 128, 0, st_>>>(tab_, kp_, order, starts, S, out_words, rec, err);
+    k_edge_walk<NW><<<blocks, 128, 0, st_>>>(tab_, kp_, order, starts, S, out_words(), rec, err);
     PG_CUDA(cudaGetLastError());
     // who emits: rounds of claim / resolve
     claimb.alloc((S + 1) * sizeof(u64));
@@ -319,9 +264,9 @@ void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
     txb.alloc((S + 1) * sizeof(u64));
     DevBuf scr2;
     scr2.alloc(scan_scratch_elems(S) * sizeof(u64));
-    device_scan(IdIn{starts, rec}, PrefixOut{idb.template as<u64>()}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
-    device_scan(TextIn{rec}, PrefixOut{txb.template as<u64>()}, S, scr2.template as<u64>(), d_cnt_ + C_MISC1, st_);
-    device_scan(Len1In{rec}, NullOut{}, S, scr2.template as<u64>(), d_cnt_ + C_MISC2, st_);
+    device_scan(IdIn{starts, rec}, ScanU64Out{idb.template as<u64>()}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
+    device_scan(TextIn{rec}, ScanU64Out{txb.template as<u64>()}, S, scr2.template as<u64>(), d_cnt_ + C_MISC1, st_);
+    device_scan_total(Len1In{rec}, S, scr2.template as<u64>(), d_cnt_ + C_MISC2, st_);
     read_counters();
     const u64 num_ed = h_cnt_[C_MISC0], text_bytes = h_cnt_[C_MISC1], n_len1 = h_cnt_[C_MISC2];
     if (num_ed >= 0xFFFFFFFFull) throw std::runtime_error("pgb200: more than 2^32 edges (the reference's ids are 32-bit)");
@@ -332,9 +277,8 @@ void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
     PG_CUDA(cudaMemsetAsync(patch_buf_.p, 0, pcap * sizeof(PatchSlot<NW>), st_));
     patch_mask_ = pcap - 1;
     textb.alloc(text_bytes + 16);
-    const bool quirk128 = prm_.flavour127 && prm_.K + 1 == 128;
-    k_edge_emit<NW><<<blocks, 128, 0, st_>>>(tab_, kp_, order, starts, S, rec, idb.template as<u64>(), txb.template as<u64>(), out_words,
-                                             textb.template as<char>(), patch_buf_.template as<PatchSlot<NW>>(), patch_mask_, quirk128, err);
+    k_edge_emit<NW><<<blocks, 128, 0, st_>>>(tab_, kp_, order, starts, S, rec, idb.template as<u64>(), txb.template as<u64>(), out_words(),
+                                             textb.template as<char>(), patch_buf_.template as<PatchSlot<NW>>(), patch_mask_, quirk128(), err);
     PG_CUDA(cudaGetLastError());
     edge_text->resize(text_bytes);
     if (text_bytes) PG_CUDA(cudaMemcpyAsync(&(*edge_text)[0], textb.p, text_bytes, cudaMemcpyDeviceToHost, st_));
@@ -348,12 +292,12 @@ void EngineT<NW>::build_edges(EdgeStats* st, std::string* edge_text) {
     st->extra_nodes = n_len1;
     // emitted = num_ed - (number of non-palindromic emitted) ; count directly
     {
-        device_scan(EmIn{rec}, NullOut{}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
+        device_scan_total(EmIn{rec}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
         read_counters();
         st->edges = h_cnt_[C_MISC0];
     }
     if (prm_.verbose) {
-        device_scan(EmNoRevIn{rec}, NullOut{}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
+        device_scan_total(EmNoRevIn{rec}, S, scr2.template as<u64>(), d_cnt_ + C_MISC0, st_);
         read_counters();
         fprintf(stderr, "[pgb200] build_edges: %llu start(s), %d claim/resolve round(s), %llu emitted start(s) without a reverse start\n",
                 (unsigned long long)S, rounds, (unsigned long long)h_cnt_[C_MISC0]);
@@ -371,11 +315,9 @@ template <int NW>
 struct VertOut {
     const Slot<NW>* slots;
     const u64* order;
-    u64* out;
+    Kmer<NW>* out;
     __device__ void operator()(u64 i, u64 prefix, u64 v) const {
-        if (!v) return;
-        Kmer<NW> k = slot_key(slots + order[i]);
-        for (int w = 0; w < NW; w++) out[prefix * NW + w] = k.w[w];
+        if (v) out[prefix] = slot_key(slots + order[i]);
     }
 };
 
@@ -385,25 +327,22 @@ void EngineT<NW>::vertices(std::string* vertex_text, uint64_t* n_vertex) {
     u64* order = order_buf_.template as<u64>();
     DevBuf scratch, outb;
     scratch.alloc(scan_scratch_elems(N) * sizeof(u64));
-    device_scan(VertIn<NW>{tab_.slots, order}, NullOut{}, N, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
+    device_scan_total(VertIn<NW>{tab_.slots, order}, N, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
     read_counters();
     u64 nv = h_cnt_[C_MISC0];
-    outb.alloc((nv + 1) * NW * sizeof(u64));
-    device_scan(VertIn<NW>{tab_.slots, order}, VertOut<NW>{tab_.slots, order, outb.template as<u64>()}, N, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
-    std::vector<u64> h(nv * NW + 1);
-    if (nv) PG_CUDA(cudaMemcpyAsync(h.data(), outb.p, nv * NW * sizeof(u64), cudaMemcpyDeviceToHost, st_));
+    outb.alloc((nv + 1) * sizeof(Kmer<NW>));
+    device_scan_finish(VertIn<NW>{tab_.slots, order}, VertOut<NW>{tab_.slots, order, outb.template as<Kmer<NW>>()}, N, scratch.template as<u64>(), st_);
+    std::vector<Kmer<NW>> h(nv + 1);
+    if (nv) PG_CUDA(cudaMemcpyAsync(h.data(), outb.p, nv * sizeof(Kmer<NW>), cudaMemcpyDeviceToHost, st_));
     sync();
-    const int out_words = prm_.flavour127 ? 4 : 2;
+    const int out_words = this->out_words();
     std::string& s = *vertex_text;
     s.clear();
     s.reserve(nv * (out_words * 17 + 1) + 16);
     char b[96];
     for (u64 i = 0; i < nv; i++) {
         int n = 0;
-        for (int w = 0; w < out_words; w++) {
-            int src = w - (out_words - NW);
-            n += snprintf(b + n, sizeof b - n, w ? " %llx" : "%llx", src >= 0 ? h[i * NW + src] : 0ull);
-        }
+        for (int w = 0; w < out_words; w++) n += snprintf(b + n, sizeof b - n, w ? " %llx" : "%llx", kout_word(h[i], w, out_words));
         b[n++] = ' ';
         s.append(b, n);
         if ((i + 1) % 8 == 0) s.push_back('\n');

@@ -151,6 +151,10 @@ public:
     // ---- state
     PgParams prm_;
     KParams<NW> kp_;
+    // Words per key in the output files (kout_word): the 127-mer build prints four at every K
+    int out_words() const { return prm_.flavour127 ? 4 : 2; }
+    // The 127-mer build's reverse complement of a (K+1) = 128-mer keeps its lowest word only (krc_ref)
+    bool quirk128() const { return prm_.flavour127 && prm_.K + 1 == 128; }
     // Three streams make pass 1 a pipeline: st_copy_ (H2D of chunk c+1) | st_dec_ (line index + decode of chunk c: all a chunk's host
     // sync waits for) | st_ (partition, aggregation, every later phase).  With the per-instance insert (PGB200_SKM=0) decode runs on st_.
     Stream st_, st_dec_;

@@ -133,6 +133,26 @@ PG_HD Kmer<NW> kprev(const Kmer<NW>& a, unsigned c, const KParams<NW>& p) {
         if (i == p.top_word) r.w[i] |= (u64)c << p.top_shift;
     return r;
 }
+// the canonical k-mer, selected word by word so that both candidates stay in registers (a select of a whole Kmer by reference puts
+// them in local memory)
+template <int NW>
+PG_D Kmer<NW> kcanon(const Kmer<NW>& f, const Kmer<NW>& rc, bool smaller) {
+    Kmer<NW> c;
+#pragma unroll
+    for (int i = 0; i < NW; i++) c.w[i] = smaller ? f.w[i] : rc.w[i];
+    return c;
+}
+// Word w of a key as the output files print it, out of out_words (EngineT::out_words): the 127-mer build prints four words at every
+// K, so a key held in two words gets two leading zero words.  Selected like kfirst: a dynamically indexed w[] lives in local memory.
+template <int NW>
+PG_HD u64 kout_word(const Kmer<NW>& a, int w, int out_words) {
+    const int src = w - (out_words - NW);
+    u64 v = 0;
+#pragma unroll
+    for (int i = 0; i < NW; i++)
+        if (i == src) v = a.w[i];
+    return v;
+}
 template <int NW>
 PG_HD unsigned klast(const Kmer<NW>& a) { return (unsigned)(a.w[NW - 1] & 3); }
 template <int NW>

@@ -21,14 +21,31 @@
 namespace pgb {
 
 struct RefGeom {
-    const u64* set_size;   // [P]
+    const u64* set_size;   // [P]; null before the sets are sized
     const u64* set_base;   // [P]
     int P;
     bool flavour127;
 };
 
+// A key's reference set and, once the sets are sized, its first slot (`base`, the set's first slot in R), the set's size and its
+// home slot in the set
+struct RefPlace {
+    u64 set, base, size, home;
+};
 template <int NW>
-__global__ void __launch_bounds__(256) k_count_sets(Table<NW> tab, int P, u64* set_count) {
+__device__ __forceinline__ RefPlace ref_place(const RefGeom& g, const Kmer<NW>& k) {
+    RefPlace p;
+    p.set = crc_hash(k) % (u64)g.P;
+    if (g.set_size) {
+        p.base = g.set_base[p.set];
+        p.size = g.set_size[p.set];
+        p.home = ref_home(k, p.size, g.flavour127);
+    }
+    return p;
+}
+
+template <int NW>
+__global__ void __launch_bounds__(256) k_count_sets(Table<NW> tab, RefGeom g, u64* set_count) {
     __shared__ unsigned s_cnt[256];
     s_cnt[threadIdx.x] = 0;
     __syncthreads();
@@ -36,10 +53,10 @@ __global__ void __launch_bounds__(256) k_count_sets(Table<NW> tab, int P, u64* s
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         const Slot<NW>* s = tab.slots + i;
         if (!slot_occupied(s)) continue;
-        atomicAdd(&s_cnt[crc_hash(slot_key(s)) % (u64)P], 1u);
+        atomicAdd(&s_cnt[ref_place(g, slot_key(s)).set], 1u);
     }
     __syncthreads();
-    if ((int)threadIdx.x < P && s_cnt[threadIdx.x]) atomicAdd(&set_count[threadIdx.x], (u64)s_cnt[threadIdx.x]);
+    if ((int)threadIdx.x < g.P && s_cnt[threadIdx.x]) atomicAdd(&set_count[threadIdx.x], (u64)s_cnt[threadIdx.x]);
 }
 
 template <int NW>
@@ -48,17 +65,15 @@ __global__ void __launch_bounds__(256) k_layout_place(Table<NW> tab, RefGeom g, 
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         const Slot<NW>* s = tab.slots + i;
         if (!slot_occupied(s)) continue;
-        Kmer<NW> k = slot_key(s);
-        int set = (int)(crc_hash(k) % (u64)g.P);
-        u64 size = g.set_size[set];
-        u64* base = R + g.set_base[set];
-        u64 pos = ref_home(k, size, g.flavour127);
+        const RefPlace p = ref_place(g, slot_key(s));
+        u64* base = R + p.base;
+        u64 pos = p.home;
         u64 r = s->aux;   // first-occurrence rank
         for (;;) {
             u64 old = atomicMin(&base[pos], r);
             if (old == EMPTY64) break;       // took a free slot
             if (old > r) r = old;            // displaced a later arrival: carry it on
-            if (++pos == size) pos = 0;
+            if (++pos == p.size) pos = 0;
         }
     }
 }
@@ -69,14 +84,12 @@ __global__ void __launch_bounds__(256) k_layout_resolve(Table<NW> tab, RefGeom g
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         const Slot<NW>* s = tab.slots + i;
         if (!slot_occupied(s)) { continue; }
-        Kmer<NW> k = slot_key(s);
-        int set = (int)(crc_hash(k) % (u64)g.P);
-        u64 size = g.set_size[set];
-        const u64* base = R + g.set_base[set];
-        u64 pos = ref_home(k, size, g.flavour127);
+        const RefPlace p = ref_place(g, slot_key(s));
+        const u64* base = R + p.base;
+        u64 pos = p.home;
         u64 r = s->aux;
-        while (base[pos] != r) { if (++pos == size) pos = 0; }
-        gpos_out[i] = g.set_base[set] + pos;
+        while (base[pos] != r) { if (++pos == p.size) pos = 0; }
+        gpos_out[i] = p.base + pos;
     }
 }
 
@@ -114,12 +127,12 @@ struct OrderOut {
 // k-mers by (set, rank) (library radix sort: plumbing outside the metric) and each set is replayed by one host thread with
 // the same put / grow rules.  Cost O(distinct); only runs when -a is absent.
 template <int NW>
-__global__ void __launch_bounds__(256) k_replay_keys(Table<NW> tab, int P, u64* sort_key, u64* sort_val, u64* cursor) {
+__global__ void __launch_bounds__(256) k_replay_keys(Table<NW> tab, RefGeom g, u64* sort_key, u64* sort_val, u64* cursor) {
     u64 n = tab.mask + 1;
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         const Slot<NW>* s = tab.slots + i;
         if (!slot_occupied(s)) continue;
-        u64 set = crc_hash(slot_key(s)) % (u64)P;
+        u64 set = ref_place(g, slot_key(s)).set;
         u64 p = atomicAdd(cursor, 1ull);
         sort_key[p] = (set << 56) | (s->aux & ((1ull << 56) - 1));   // rank < 2^56 (read ordinal < 2^40)
         sort_val[p] = i;
@@ -193,14 +206,25 @@ void EngineT<NW>::build_layout() {
     settle_timing();
     read_counters();
     n_nodes_ = h_cnt_[C_DISTINCT];
+    const u64 N = n_nodes_;
+    // order[] from R (R[reference slot] = the ktab slot of the key there, EMPTY64 where the slot is free): the occupied slots in order
+    auto order_from = [&](u64* R, u64 total) {
+        DevBuf scratch;
+        order_buf_.alloc((N + 1) * sizeof(u64));
+        scratch.alloc(scan_scratch_elems(total) * sizeof(u64));
+        device_scan(OccIn{R}, OrderOut<NW>{R, order_buf_.template as<u64>(), tab_.slots}, total, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
+        read_counters();
+        if (h_cnt_[C_MISC0] != N) throw std::runtime_error("pgb200: internal error: layout lost k-mers");
+    };
     std::vector<u64> set_size(P), set_base(P);
     DevBuf d_geom;
     d_geom.alloc(3 * P * sizeof(u64));
     u64* d_size = d_geom.template as<u64>();
     u64* d_base = d_size + P;
     u64* d_count = d_base + P;
+    const RefGeom unsized{nullptr, nullptr, P, prm_.flavour127 != 0};
     PG_CUDA(cudaMemsetAsync(d_count, 0, P * sizeof(u64), st_));
-    k_count_sets<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, P, d_count);
+    k_count_sets<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, unsized, d_count);
     PG_CUDA(cudaGetLastError());
     std::vector<u64> cnt(P);
     PG_CUDA(cudaMemcpyAsync(cnt.data(), d_count, P * sizeof(u64), cudaMemcpyDeviceToHost, st_));
@@ -215,12 +239,11 @@ void EngineT<NW>::build_layout() {
         // Dynamic growth: replay every set's growth history (see above)
         for (int i = 0; i < P; i++)
             if (cnt[i] >= 0xFFFFFFF0ull) throw std::runtime_error("pgb200: a dynamic reference set would exceed 2^32 entries; use -a");
-        const u64 N = n_nodes_;
         DevBuf kb, vb, kb2, vb2, curb, tmpb, keysb;
         kb.alloc((N + 1) * sizeof(u64)); vb.alloc((N + 1) * sizeof(u64)); kb2.alloc((N + 1) * sizeof(u64)); vb2.alloc((N + 1) * sizeof(u64));
         curb.alloc(sizeof(u64));
         PG_CUDA(cudaMemsetAsync(curb.p, 0, sizeof(u64), st_));
-        k_replay_keys<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, P, kb.template as<u64>(), vb.template as<u64>(), curb.template as<u64>());
+        k_replay_keys<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, unsized, kb.template as<u64>(), vb.template as<u64>(), curb.template as<u64>());
         PG_CUDA(cudaGetLastError());
         size_t tmp_bytes = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, kb.template as<u64>(), kb2.template as<u64>(), vb.template as<u64>(), vb2.template as<u64>(), N, 0, 64, st_);
@@ -248,19 +271,14 @@ void EngineT<NW>::build_layout() {
         for (int i = 0; i < P; i++)
             for (u64 j = 0; j < set_size[i]; j++)
                 if (slots[i][j]) h_gpos[first[i] + slots[i][j] - 1] = set_base[i] + j;
-        DevBuf gposb, Rb, scratch;
+        DevBuf gposb, Rb;
         gposb.alloc((N + 1) * sizeof(u64));
         PG_CUDA(cudaMemcpyAsync(gposb.p, h_gpos.data(), N * sizeof(u64), cudaMemcpyHostToDevice, st_));
         Rb.alloc(total * sizeof(u64));
         PG_CUDA(cudaMemsetAsync(Rb.p, 0xFF, total * sizeof(u64), st_));
         k_fill_R<<<n_sm_ * 8, 256, 0, st_>>>(vb2.template as<u64>(), gposb.template as<u64>(), N, Rb.template as<u64>());
         PG_CUDA(cudaGetLastError());
-        order_buf_.alloc((N + 1) * sizeof(u64));
-        scratch.alloc(scan_scratch_elems(total) * sizeof(u64));
-        device_scan(OccIn{Rb.template as<u64>()}, OrderOut<NW>{Rb.template as<u64>(), order_buf_.template as<u64>(), tab_.slots}, total,
-                    scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
-        read_counters();
-        if (h_cnt_[C_MISC0] != N) throw std::runtime_error("pgb200: internal error: dynamic layout replay lost k-mers");
+        order_from(Rb.template as<u64>(), total);
         return;
     }
     u64 total = 0;
@@ -271,7 +289,7 @@ void EngineT<NW>::build_layout() {
     PG_CUDA(cudaMemcpyAsync(d_size, set_size.data(), P * sizeof(u64), cudaMemcpyHostToDevice, st_));
     PG_CUDA(cudaMemcpyAsync(d_base, set_base.data(), P * sizeof(u64), cudaMemcpyHostToDevice, st_));
 
-    DevBuf Rb, gposb, scratch;
+    DevBuf Rb, gposb;
     Rb.alloc(total * sizeof(u64));
     gposb.alloc(cap_ * sizeof(u64));
     PG_CUDA(cudaMemsetAsync(Rb.p, 0xFF, total * sizeof(u64), st_));
@@ -281,11 +299,7 @@ void EngineT<NW>::build_layout() {
     k_layout_resolve<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, g, R, gposb.template as<u64>());
     k_layout_fill<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, gposb.template as<u64>(), R);
     PG_CUDA(cudaGetLastError());
-    order_buf_.alloc((n_nodes_ + 1) * sizeof(u64));
-    scratch.alloc(scan_scratch_elems(total) * sizeof(u64));
-    device_scan(OccIn{R}, OrderOut<NW>{R, order_buf_.template as<u64>(), tab_.slots}, total, scratch.template as<u64>(), d_cnt_ + C_MISC0, st_);
-    read_counters();
-    if (h_cnt_[C_MISC0] != n_nodes_) throw std::runtime_error("pgb200: internal error: layout lost k-mers");
+    order_from(R, total);
 }
 
 // ---------------------------------------------------------------- parity dump (record format documented in include/pregraph_b200.h)
@@ -298,8 +312,7 @@ __global__ void k_dump_nodes(Table<NW> tab, const u64* order, u64 n, int out_wor
         u64 p = s->payload;
         unsigned char* o = out + i * rec;
         for (int w = 0; w < out_words; w++) {
-            int src = w - (out_words - NW);
-            u64 v = src >= 0 ? k.w[src] : 0ull;
+            u64 v = kout_word(k, w, out_words);
             for (int b = 0; b < 8; b++) o[w * 8 + b] = (unsigned char)(v >> (8 * b));
         }
         o += out_words * 8;
@@ -312,11 +325,10 @@ __global__ void k_dump_nodes(Table<NW> tab, const u64* order, u64 n, int out_wor
 template <int NW>
 void EngineT<NW>::dump_nodes(void* host_out) {
     if (!order_buf_.p) throw std::runtime_error("pgb200: dump_nodes before build_layout");
-    const int out_words = prm_.flavour127 ? 4 : 2;
-    const size_t rec = out_words * 8 + 10;
+    const size_t rec = out_words() * 8 + 10;
     DevBuf d;
     d.alloc(n_nodes_ * rec);
-    k_dump_nodes<NW><<<n_sm_ * 4, 256, 0, st_>>>(tab_, order_buf_.template as<u64>(), n_nodes_, out_words, d.template as<unsigned char>());
+    k_dump_nodes<NW><<<n_sm_ * 4, 256, 0, st_>>>(tab_, order_buf_.template as<u64>(), n_nodes_, out_words(), d.template as<unsigned char>());
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cudaMemcpyAsync(host_out, d.p, n_nodes_ * rec, cudaMemcpyDeviceToHost, st_));
     sync();

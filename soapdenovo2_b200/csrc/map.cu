@@ -76,16 +76,6 @@ PG_D KPair<NW> first_kmer(const u64* __restrict__ w, u64 b, const KParams<NW>& k
     return k;
 }
 
-// the canonical k-mer, selected word by word so that both candidates stay in registers (a select of a whole Kmer by reference puts
-// them in local memory)
-template <int NW>
-PG_D Kmer<NW> kcanon(const Kmer<NW>& f, const Kmer<NW>& rc, bool smaller) {
-    Kmer<NW> c;
-#pragma unroll
-    for (int i = 0; i < NW; i++) c.w[i] = smaller ? f.w[i] : rc.w[i];
-    return c;
-}
-
 // The canonical form of k-mer j of the bases at w (bases b + j .. b + j + K - 1).  k holds k-mer j - 1 and is rolled on by one base,
 // except at the first k-mer j0 of a loop, which first_kmer built.  *smaller: the forward k-mer is the smaller (isSmaller).
 template <int NW>
@@ -247,12 +237,6 @@ __global__ void __launch_bounds__(MAP_LONG_THREADS) k_map_long(Table<NW> t, KPar
     }
 }
 
-// words of a read packed at its own length
-struct WordsOfLen {
-    const u32* lens;
-    __device__ u64 operator()(u64 i) const { return (lens[i] + 31u) / 32u; }
-};
-
 // strided decode output (stride words per read) -> packed at each read's own length, read r at ofs[r]; one thread per input word
 __global__ void __launch_bounds__(256) k_pack_reads(const u64* __restrict__ in, int stride, const u32* __restrict__ lens, const u64* __restrict__ ofs,
                                                     u64 n, u64* __restrict__ packed) {
@@ -331,7 +315,7 @@ public:
         pack_scan_.ensure(scan_scratch_elems(n) * sizeof(u64));
         pack_words_.ensure(n * S * sizeof(u64));
         u64* ofs = pack_ofs_.as<u64>();
-        device_scan(WordsOfLen{read_lens_.as<u32>()}, ScanU64Out{ofs}, n, pack_scan_.as<u64>(), ofs + n, st_);
+        device_scan(ScanWordsOfLen{read_lens_.as<u32>()}, ScanU64Out{ofs}, n, pack_scan_.as<u64>(), ofs + n, st_);
         k_pack_reads<<<(unsigned)std::min<u64>((n * S + 255) / 256, (u64)n_sm_ * 64), 256, 0, st_>>>(read_words_.as<u64>(), S, read_lens_.as<u32>(), ofs, n,
                                                                                              pack_words_.as<u64>());
         PG_CUDA(cudaGetLastError());

@@ -85,9 +85,8 @@ __global__ void __launch_bounds__(128) k_pass2(Table<NW> tab, KParams<NW> kp, co
             fwd = knext(fwd, c, kp);
             rc = kprev(rc, c ^ 2u, kp);
             if (i < K - 1) continue;
-            bool sm = kless(fwd, rc);
-            Kmer<NW> canon = sm ? fwd : rc;
-            u64 slot = table_find(tab, canon);
+            const bool sm = !kless(rc, fwd);
+            u64 slot = table_find(tab, kcanon(fwd, rc, sm));
             if (slot == ~0ull) { atomicAdd(err, 1ull); stop = true; break; }
             const Slot<NW>* nd = tab.slots + slot;
             u64 p = nd->payload;
@@ -150,17 +149,6 @@ __global__ void __launch_bounds__(128) k_write_paths(const u32* __restrict__ len
     }
 }
 
-struct RecIn {
-    const u32* reclen;
-    __device__ u64 operator()(u64 i) const { return reclen[i]; }
-};
-struct RecOut {
-    u64* off;
-    __device__ void operator()(u64 i, u64 prefix, u64) const { off[i] = prefix; }
-};
-struct CountOnly {
-    __device__ void operator()(u64, u64, u64) const {}
-};
 struct ArcOccIn {
     const ArcSlot* t;
     __device__ u64 operator()(u64 i) const { return t[i].key != EMPTY64; }
@@ -176,7 +164,6 @@ void EngineT<NW>::pass2(Pass2Stats* st, std::string* prearc_text, std::string* p
     if (!patch_buf_.p) throw std::runtime_error("pgb200: pass2 before build_edges");
     const int K = prm_.K;
     const int stride = prm_.max_rd_len - K + 1 + 1;   // path entries + one bookkeeping word
-    const bool quirk128 = prm_.flavour127 && K + 1 == 128;
     u64 total_ord = 0, max_rec = 0;
     for (auto& c : chunks_) {
         if (c.n_rec) total_ord = std::max(total_ord, c.ord_base + (c.n_rec - 1) * c.ord_stride + 1);
@@ -211,10 +198,10 @@ void EngineT<NW>::pass2(Pass2Stats* st, std::string* prearc_text, std::string* p
         else pb = shared_path.template as<u32>();
         unsigned blocks = (unsigned)std::min<u64>((c.n_rec + 127) / 128, (u64)n_sm_ * 32);
         size_t smem = (size_t)128 * W64_ * sizeof(u64);
-        int use_tma = smem <= 48 * 1024 && !getenv("PGB200_NO_TMA");
+        int use_tma = smem <= 48 * 1024;   // longer reads: the unstaged loop
         k_pass2<NW><<<blocks, 128, use_tma ? smem : 0, st_>>>(tab_, kp_, c.words, c.len, c.n_rec, W64_, c.ord_base, c.ord_stride, stride, pb,
                                              reclenb.template as<u32>(), prm_.repsTie, patch_buf_.template as<PatchSlot<NW>>(), patch_mask_,
-                                             quirk128, arcs, acap - 1, markb.template as<u32>(), d_cnt_, errb.template as<u64>(), use_tma);
+                                             quirk128(), arcs, acap - 1, markb.template as<u32>(), d_cnt_, errb.template as<u64>(), use_tma);
         PG_CUDA(cudaGetLastError());
     }
     u64 herr[2];
@@ -227,11 +214,11 @@ void EngineT<NW>::pass2(Pass2Stats* st, std::string* prearc_text, std::string* p
     // ---- arcs: compact, copy, order by (from asc, first-seen rank desc), print (output_arcs)
     scratch.alloc(scan_scratch_elems(std::max<u64>(acap, total_ord + 1)) * sizeof(u64));
     DevBuf compb;
-    device_scan(ArcOccIn{arcs}, CountOnly{}, acap, scratch.template as<u64>(), d_cnt_ + C_MISC1, st_);
+    device_scan_total(ArcOccIn{arcs}, acap, scratch.template as<u64>(), d_cnt_ + C_MISC1, st_);
     read_counters();
     u64 n_arcs = h_cnt_[C_MISC1];
     compb.alloc((n_arcs + 1) * sizeof(ArcSlot));
-    device_scan(ArcOccIn{arcs}, ArcCompactOut{arcs, compb.template as<ArcSlot>()}, acap, scratch.template as<u64>(), d_cnt_ + C_MISC1, st_);
+    device_scan_finish(ArcOccIn{arcs}, ArcCompactOut{arcs, compb.template as<ArcSlot>()}, acap, scratch.template as<u64>(), st_);
     std::vector<ArcSlot> h(n_arcs);
     if (n_arcs) PG_CUDA(cudaMemcpyAsync(h.data(), compb.p, n_arcs * sizeof(ArcSlot), cudaMemcpyDeviceToHost, st_));
     sync();
@@ -257,7 +244,7 @@ void EngineT<NW>::pass2(Pass2Stats* st, std::string* prearc_text, std::string* p
     mark_text->clear();
     if (prm_.repsTie) {
         recoffb.alloc((total_ord + 1) * sizeof(u64));
-        device_scan(RecIn{reclenb.template as<u32>()}, RecOut{recoffb.template as<u64>()}, total_ord, scratch.template as<u64>(), d_cnt_ + C_MISC2, st_);
+        device_scan(ScanU32In{reclenb.template as<u32>()}, ScanU64Out{recoffb.template as<u64>()}, total_ord, scratch.template as<u64>(), d_cnt_ + C_MISC2, st_);
         read_counters();
         u64 pbytes = h_cnt_[C_MISC2];
         DevBuf outb;

@@ -90,15 +90,6 @@ __global__ void __launch_bounds__(256) k_fg_count(const uint4* __restrict__ text
     if (lane == 0 && nul) atomicAdd((unsigned long long*)&slots[FG_NUL], (unsigned long long)nul);
 }
 
-struct FgTileIn {
-    const u32* a;
-    __device__ u64 operator()(u64 i) const { return a[i]; }
-};
-struct U32PrefixOut {
-    u32* a;
-    __device__ void operator()(u64 i, u64 prefix, u64) const { a[i] = (u32)prefix; }
-};
-
 __global__ void __launch_bounds__(256) k_fg_nlpos(const uint4* __restrict__ text, u64 nbytes, u64 n_tiles, const u32* __restrict__ tile_base,
                                                   u32* __restrict__ nl) {
     const int lane = threadIdx.x & 31;
@@ -348,11 +339,6 @@ __global__ void __launch_bounds__(256) k_fg_fix_len(const unsigned char* __restr
     }
 }
 
-struct FgWordsIn {
-    const u32* lens;
-    __device__ u64 operator()(u64 i) const { return (lens[i] + 31u) / 32u; }
-};
-
 __global__ void __launch_bounds__(256) k_fg_fix_decode(const unsigned char* __restrict__ text, const u32* __restrict__ pstart, const u8* __restrict__ role,
                                                        const u32* __restrict__ hdr, u64 n_hdr, u64 np, u32 cutoff, int reverse, const u32* __restrict__ redo,
                                                        const u64* slots, const u32* __restrict__ lens, const u64* __restrict__ wofs, u64* __restrict__ words) {
@@ -449,7 +435,7 @@ size_t FgetsReader::read(const unsigned char* d_text, size_t nbytes, int fastq, 
     const uint4* t16 = reinterpret_cast<const uint4*>(d_text);
     k_fg_count<<<blocks(n_tiles, 8, 16), 256, 0, st>>>(t16, (u64)nbytes, n_tiles, tile_cnt, slots);
     PG_CUDA(cudaGetLastError());
-    device_scan(FgTileIn{tile_cnt}, U32PrefixOut{tile_base}, n_tiles, tmp, slots + FG_NL, st);
+    device_scan(ScanU32In{tile_cnt}, ScanU32Out{tile_base}, n_tiles, tmp, slots + FG_NL, st);
     unsigned char* h_last = reinterpret_cast<unsigned char*>(h + FG_SLOTS);
     PG_CUDA(cudaMemcpyAsync(h_last, d_text + nbytes - 1, 1, cudaMemcpyDeviceToHost, st));
     PG_CUDA(cudaMemcpyAsync(h, slots, FG_SLOTS * sizeof(u64), cudaMemcpyDeviceToHost, st));
@@ -462,7 +448,7 @@ size_t FgetsReader::read(const unsigned char* d_text, size_t nbytes, int fastq, 
     PG_CUDA(cudaGetLastError());
     const FgLines L{nl_.as<u32>(), n_nl, (u64)nbytes};
     lpb_.ensure(n_lines * sizeof(u32) + 16);
-    device_scan(FgLinePiecesIn{L, P}, U32PrefixOut{lpb_.as<u32>()}, n_lines, tmp, slots + FG_PIECES, st);
+    device_scan(FgLinePiecesIn{L, P}, ScanU32Out{lpb_.as<u32>()}, n_lines, tmp, slots + FG_PIECES, st);
     PG_CUDA(cudaMemcpyAsync(h, slots, FG_SLOTS * sizeof(u64), cudaMemcpyDeviceToHost, st));
     PG_CUDA(cudaStreamSynchronize(st));
 
@@ -509,7 +495,7 @@ size_t FgetsReader::read(const unsigned char* d_text, size_t nbytes, int fastq, 
         k_fg_fix_len<<<(unsigned)n_sm * 8, 256, 0, st>>>(d_text, pstart, role, hdr, n_hdr, np, (u32)cutoff, redo_.as<u32>(), slots, d_lens);
         PG_CUDA(cudaGetLastError());
     }
-    device_scan(FgWordsIn{d_lens}, ScanU64Out{wofs}, n_rec, tmp, wofs + n_rec, st);   // wofs[n_rec]: the word total, read as r + 1
+    device_scan(ScanWordsOfLen{d_lens}, ScanU64Out{wofs}, n_rec, tmp, wofs + n_rec, st);   // wofs[n_rec]: the word total, read as r + 1
     PG_CUDA(cudaMemcpyAsync(slots + FG_WORDS, wofs + n_rec, sizeof(u64), cudaMemcpyDeviceToDevice, st));
     k_fg_tail<<<1, 1, 0, st>>>(d_text, (u64)nbytes, pstart, role, hdr, n_hdr, np, (u32)P, fastq, at_eof ? 1 : 0, slots);
     PG_CUDA(cudaGetLastError());

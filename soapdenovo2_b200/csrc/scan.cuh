@@ -1,7 +1,8 @@
 // scan.cuh -- device-wide exclusive prefix sum with fused input/output functors (hand-written, no CUB).
 //
-// Used for: newline -> line index (decode.cu), occupancy -> position in reference iteration order (layout.cu),
-// per-edge text lengths / edge ids (edges.cu), per-read record offsets (pass2.cu).
+// Used for: newline counts -> line index (decode.cu, reader.cu), bucket counts -> record offsets (skm.cu), read lengths -> packed
+// word offsets (map.cu, reader.cu), occupancy -> position in reference iteration order (layout.cu), tip candidates (tips.cu), edge
+// starts, ids, text offsets and vertices (edges.cu), arc compaction and per-read path record offsets (pass2.cu).
 // Three launches per level: tile sums -> (recursive) scan of the tile sums -> rescan tiles with their base.
 // A tile is SCAN_THREADS x SCAN_ITEMS consecutive elements; thread t owns items [t*ITEMS, (t+1)*ITEMS) so a tile needs one
 // block-wide scan (the per-thread runs are contiguous 256 B pieces for 16-byte elements: sector-efficient streaming).
@@ -96,13 +97,27 @@ static __global__ void __launch_bounds__(SCAN_THREADS) k_scan_small(u64* a, u64 
     if (threadIdx.x == 0 && total_out) *total_out = running;
 }
 
+// The common inputs and outputs: an array of counts in, the exclusive prefix out at the same index
+struct ScanU32In {
+    const u32* a;
+    __device__ u64 operator()(u64 i) const { return a[i]; }
+};
 struct ScanU64In {
     const u64* a;
     __device__ u64 operator()(u64 i) const { return a[i]; }
 };
+struct ScanU32Out {
+    u32* a;
+    __device__ void operator()(u64 i, u64 prefix, u64) const { a[i] = (u32)prefix; }
+};
 struct ScanU64Out {
     u64* a;
     __device__ void operator()(u64 i, u64 prefix, u64) const { a[i] = prefix; }
+};
+// 64-bit words of a 2-bit packed read of lens[i] bases
+struct ScanWordsOfLen {
+    const u32* lens;
+    __device__ u64 operator()(u64 i) const { return (lens[i] + 31u) / 32u; }
 };
 
 // scratch: caller-provided device buffer of at least scan_scratch_elems(n) u64.
@@ -130,7 +145,8 @@ void device_scan(In in, Out out, u64 n, u64* scratch, u64* d_total, cudaStream_t
 }
 
 // Split form for the case "total first, then (after the caller has sized its outputs) the prefixes": phase 1 leaves the scanned
-// tile bases in `scratch`, phase 2 reuses them -- the input is read twice in total instead of four times.
+// tile bases in `scratch`, phase 2 reuses them -- the input is read twice in total instead of four times.  Nothing the input reads
+// and nothing in `scratch` may change between the two calls.  device_scan_total alone is a device-wide sum.
 template <class In>
 void device_scan_total(In in, u64 n, u64* scratch, u64* d_total, cudaStream_t st) {
     if (n == 0) { cudaMemsetAsync(d_total, 0, sizeof(u64), st); return; }

@@ -44,15 +44,6 @@ __global__ void __launch_bounds__(SKM_PART_THREADS) k_skm_count(SkmGeom g, const
     }
 }
 
-struct BucketCntIn {
-    const u32* a;
-    __device__ u64 operator()(u64 i) const { return a[i]; }
-};
-struct BucketOffOut {
-    u32* a;
-    __device__ void operator()(u64 i, u64 prefix, u64) const { a[i] = (u32)prefix; }
-};
-
 // ------------------------------------------------------------------------------------------------ partition: publish + scatter
 struct SkmSendArgs {
     u32 n_buckets;
@@ -393,7 +384,7 @@ void EngineT<NW>::skm_feed_chunk(size_t ci) {
     k_skm_count<<<(unsigned)std::min<u64>((ch.n_rec + skm_part_threads_ - 1) / skm_part_threads_, (u64)n_sm_ * 16), skm_part_threads_, ring, st_>>>(skm_geom_, ch.words, ch.len, ch.n_rec, W64_, skm_cnt_.template as<u32>(), side, nruns);
     PG_CUDA(cudaGetLastError());
     SkmScratch* sc = skm_scratch_.template as<SkmScratch>();
-    device_scan(BucketCntIn{skm_cnt_.template as<u32>()}, BucketOffOut{skm_segoff_.template as<u32>()}, (u64)B, skm_scan_.template as<u64>(),
+    device_scan(ScanU32In{skm_cnt_.template as<u32>()}, ScanU32Out{skm_segoff_.template as<u32>()}, (u64)B, skm_scan_.template as<u64>(),
                 &sc->blob_total, st_);
     SkmSendArgs a;
     a.n_buckets = B;

@@ -11,6 +11,7 @@
 //   removeSingleTips :363-399 one sweep in iteration order over `!linear && !deleted && single` nodes, THIN = 1 (only when -d 0)
 //   removeMinorTips  :414-488 sweeps in iteration order over `!linear && !deleted` nodes until a sweep clips nothing
 //   thread_mark      :532-564 re-mark 1-in-1-out nodes linear (skips deleted / already linear)
+// The walk itself is walk.cuh's, shared with the edges.
 //
 // Why this can be parallel and still exact:
 //   THIN pass.  Chain nodes are linear AND single and are never written; start nodes are single dead ends whose only link
@@ -25,6 +26,7 @@
 //   committed candidate saw precisely the state the sequential loop would have shown it.
 #include "engine_impl.cuh"
 #include "scan.cuh"
+#include "walk.cuh"
 #include <algorithm>
 
 namespace pgb {
@@ -32,60 +34,31 @@ namespace pgb {
 struct TipRec {
     u64 n1_slot;
     u64 out_slot;
-    u32 code;     // link to clear at out: bit 2 = right side, bits 0..1 = base
+    u32 code;     // bits 0..2: the link to clear at out (walk.cuh); 8 makes out linear, 16 makes it a dead end, 32 no out (THIN)
     u32 state;    // THIN: 0 pending, 1 done.   minor: decision 0 none / 1 clip / 2 isolated
 };
 
-template <int NW>
-struct Walk {
-    u64 out_slot;
-    int sm;
-    unsigned ch;      // firstCharInKmer(pre_word)
-    int status;       // 0 = gave up (too long / not a dead end), 1 = reached `out`, -1 = lookup failed
-};
-
-template <int NW>
-__device__ __forceinline__ void canon_of(const Kmer<NW>& w, const KParams<NW>& kp, Kmer<NW>& word, Kmer<NW>& bal, int& sm) {
-    Kmer<NW> b = krc_n(w, kp.K);
-    if (kless(b, w)) { word = b; bal = w; sm = 0; } else { word = w; bal = b; sm = 1; }   // KmerLarger(word, bal) -> swap
+// A tip starts at a dead end, (in, out) = (0, 1) or (1, 0), and leaves through its only link; ~0u: not a dead end
+__device__ __forceinline__ unsigned tip_link(u64 p) {
+    if (pl_nl(p) == 0 && pl_nr(p) == 1) return (unsigned)pl_first_r(p);
+    if (pl_nl(p) == 1 && pl_nr(p) == 0) return 4u | (unsigned)pl_first_l(p);
+    return ~0u;
 }
 
-// visit(slot) is called for every node the walk READS (start, chain, out).
-template <int NW, class Visit>
-__device__ Walk<NW> tip_walk(const Table<NW>& tab, const KParams<NW>& kp, u64 n1_slot, int cut, bool THIN, Visit visit) {
-    Walk<NW> r;
-    r.status = 0; r.out_slot = 0; r.sm = 1; r.ch = 0;
-    const Slot<NW>* n1 = tab.slots + n1_slot;
-    u64 p1 = n1->payload;
-    visit(n1_slot);
-    int in = pl_nl(p1), on = pl_nr(p1);
-    Kmer<NW> pre, word;
-    if (in == 0 && on == 1) { pre = slot_key(n1); word = knext(pre, (unsigned)pl_first_r(p1), kp); }
-    else if (in == 1 && on == 0) { pre = krc_n(slot_key(n1), kp.K); word = knext(pre, (unsigned)pl_first_l(p1) ^ 2u, kp); }
-    else return r;
-    int count = 1;
-    Kmer<NW> cw, cb;
-    int sm;
-    canon_of(word, kp, cw, cb, sm);
-    u64 os = table_find(tab, cw);
-    if (os == ~0ull) { r.status = -1; return r; }
-    visit(os);
-    u64 po = tab.slots[os].payload;
-    while (po & PL_LINEAR) {
-        count++;
-        if (THIN && !(po & PL_SINGLE)) break;
-        if (count > cut) return r;
-        if (sm) { pre = cw; word = knext(pre, (unsigned)pl_first_r(po), kp); }
-        else { pre = cb; word = knext(pre, (unsigned)pl_first_l(po) ^ 2u, kp); }
-        canon_of(word, kp, cw, cb, sm);
-        os = table_find(tab, cw);
-        if (os == ~0ull) { r.status = -1; return r; }
-        visit(os);
-        po = tab.slots[os].payload;
+// clipTipFromNode's walk: the THIN pass stops at the first linear node that is not single, and a walk gives up when its count of
+// nodes (the start included) passes `cut`.  read(slot) sees each linear node the walk reads.
+template <class Read>
+struct TipVisit {
+    int cut;
+    bool thin;
+    Read read;
+    template <int NW>
+    __device__ int operator()(u32 i, u64 slot, int, const Kmer<NW>&, u64 po) {
+        read(slot);
+        if (thin && !(po & PL_SINGLE)) return WALK_STOP;
+        return (int)i + 1 > cut ? WALK_GIVE_UP : WALK_GO;
     }
-    r.status = 1; r.out_slot = os; r.sm = sm; r.ch = kfirst(pre, kp);
-    return r;
-}
+};
 
 struct NoVisit {
     __device__ void operator()(u64) const {}
@@ -115,13 +88,17 @@ template <int NW>
 __global__ void __launch_bounds__(256) k_thin_walk(Table<NW> tab, KParams<NW> kp, const u64* order, const u64* cand, u64 n, int cut, TipRec* rec, u64* err) {
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         u64 s1 = order[cand[i]];
-        Walk<NW> w = tip_walk(tab, kp, s1, cut, true, NoVisit());
         TipRec r;
-        r.n1_slot = s1; r.out_slot = w.out_slot;
-        r.code = w.sm ? w.ch : (4u | (w.ch ^ 2u));   // dislink2prevUncertain: smaller ? l[ch] : r[ch^2]
-        r.state = w.status == 1 ? 0u : 1u;            // too long -> nothing to do
-        if (w.status != 1) r.code |= 32u;             // no `out` node: out_slot is meaningless (k_thin_unmark must not follow it)
-        if (w.status < 0) atomicAdd(err, 1ull);
+        r.n1_slot = s1; r.out_slot = 0;
+        r.code = 32u;   // no `out` node (too long, or not a tip): nothing to do, and k_thin_unmark must not follow out_slot
+        r.state = 1u;
+        const unsigned link = tip_link(tab.slots[s1].payload);
+        if (link != ~0u) {
+            TipVisit<NoVisit> tv{cut, true, NoVisit()};
+            WalkEnd<NW> w = unipath_walk(tab, kp, s1, link, tv);
+            if (w.status == WALK_REACHED) { r.out_slot = w.slot; r.code = w.rev; r.state = 0u; }
+            if (w.status == WALK_MISS) atomicAdd(err, 1ull);
+        }
         rec[i] = r;
     }
 }
@@ -149,9 +126,7 @@ __global__ void __launch_bounds__(256) k_thin_commit(Table<NW> tab, const u64* c
         tips++;
         n1->payload |= PL_DELETED;
         if (pl_nl(po) + pl_nr(po) == 1) { out->payload = po | PL_DELETED; continue; }
-        unsigned c = rec[i].code;
-        po = (c & 4u) ? pl_clear_r(po, c & 3u) : pl_clear_l(po, c & 3u);
-        out->payload = po & ~PL_LINEAR;
+        out->payload = link_clear(po, rec[i].code & 7u) & ~PL_LINEAR;
     }
     if (tips) atomicAdd(&counters[C_MISC0], (u64)tips);
     if (pending) atomicAdd(&counters[C_MISC1], (u64)pending);
@@ -195,19 +170,24 @@ __device__ MinorDecision<NW> minor_decide(const Table<NW>& tab, const KParams<NW
     MinorDecision<NW> d;
     d.decision = 0; d.out_slot = 0; d.code = 0; d.makes_linear = false; d.makes_deadend = false;
     u64 p1 = tab.slots[s1].payload;
-    if (p1 & (PL_LINEAR | PL_DELETED)) { visit(s1); return d; }   // no longer a candidate at its turn
-    Walk<NW> w = tip_walk(tab, kp, s1, cut, false, visit);
-    if (w.status < 0) { atomicAdd(err, 1ull); return d; }
-    if (w.status == 0) return d;
-    d.out_slot = w.out_slot;
-    u64 po = tab.slots[w.out_slot].payload;
+    visit(s1);
+    if (p1 & (PL_LINEAR | PL_DELETED)) return d;   // no longer a candidate at its turn
+    const unsigned link = tip_link(p1);
+    if (link == ~0u) return d;
+    TipVisit<Visit> tv{cut, false, visit};
+    WalkEnd<NW> w = unipath_walk(tab, kp, s1, link, tv);
+    if (w.status == WALK_MISS) { atomicAdd(err, 1ull); return d; }
+    if (w.status == WALK_GAVE_UP) return d;
+    visit(w.slot);
+    d.out_slot = w.slot;
+    u64 po = tab.slots[w.slot].payload;
     if (pl_nl(po) + pl_nr(po) == 1) { d.decision = 2; return d; }
-    unsigned mx = 0, mine;
-    if (w.sm) { for (int c = 0; c < 4; c++) mx = max(mx, pl_l(po, c)); mine = pl_l(po, w.ch); d.code = w.ch; }
-    else { for (int c = 0; c < 4; c++) mx = max(mx, pl_r(po, c)); mine = pl_r(po, w.ch ^ 2u); d.code = 4u | (w.ch ^ 2u); }
-    if (mine < mx) {
+    unsigned mx = 0;
+    for (unsigned c = 0; c < 4; c++) mx = max(mx, link_count(po, (w.rev & 4u) | c));
+    d.code = w.rev;
+    if (link_count(po, w.rev) < mx) {
         d.decision = 1;
-        u64 pn = (d.code & 4u) ? pl_clear_r(po, d.code & 3u) : pl_clear_l(po, d.code & 3u);
+        u64 pn = link_clear(po, w.rev);
         int in = pl_nl(pn), on = pl_nr(pn);
         d.makes_linear = (in == 1 && on == 1);
         // out turns into a NEW dead end that the same sweep will visit if it lies further down the iteration order
@@ -276,8 +256,7 @@ __global__ void __launch_bounds__(128) k_minor_commit(Table<NW> tab, const u64* 
         atomicAdd(&ctl[2], 1ull);              // tip_c++ / flag++
         n1->payload |= PL_DELETED;
         if (r.state == 2) { out->payload |= PL_DELETED; continue; }
-        u64 po = out->payload;
-        po = (r.code & 4u) ? pl_clear_r(po, r.code & 3u) : pl_clear_l(po, r.code & 3u);
+        u64 po = link_clear(out->payload, r.code & 7u);
         if (r.code & 8u) po |= PL_LINEAR;
         out->payload = po;
         if (r.code & 16u) {
@@ -285,10 +264,6 @@ __global__ void __launch_bounds__(128) k_minor_commit(Table<NW> tab, const u64* 
             if (b > me) { u64 k = atomicAdd(&ctl[3], 1ull); extra[k] = b; }   // visited later in this very sweep
         }
     }
-}
-
-__global__ void k_fill_u64(u64* p, u64 n, u64 v) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) p[i] = v;
 }
 
 template <int NW>
