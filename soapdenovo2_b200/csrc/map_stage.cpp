@@ -29,9 +29,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <exception>
+#include <future>
 #include <memory>
 #include <stdexcept>
-#include <thread>
 #include <getopt.h>
 #include <zlib.h>
 
@@ -59,12 +59,6 @@ int min_overlap(const std::string& prefix) {   // getMinOverlap, map.c:48-76
     return K;
 }
 
-FILE* ckopen(const std::string& name, const char* mode) {
-    FILE* fp = fopen(name.c_str(), mode);
-    if (!fp) fail("Cannot open %s. Now exit to system...", name.c_str());   // check.c:30-34
-    return fp;
-}
-
 // The kept contigs of <prefix>.contig, their bases packed 2 bits each into one stream (LSB first)
 struct Contigs {
     std::vector<u64> packed, off{0};
@@ -72,12 +66,8 @@ struct Contigs {
     u64 n_kmers = 0;
 };
 Contigs read_contigs(const std::string& prefix, int K) {
-    const std::string name = prefix + ".contig";
-    FILE* fp = ckopen(name, "r");
-    std::string text;
-    char buf[1 << 16];
-    size_t got;
-    while ((got = fread(buf, 1, sizeof buf, fp)) > 0) text.append(buf, got);
+    FILE* fp = ckopen(prefix + ".contig", "r");
+    const std::string text = read_whole_file(fp);
     fclose(fp);
     // readseqpar (readseq1by1.c:225-277): record count and the length / name extremes, from the line lengths
     long long num = -1;
@@ -177,46 +167,26 @@ struct Reads {
     std::vector<int> lib;   // index into MapPlan::libs / long_libs
 };
 
-// One file's reads, appended to *words / *lens, each cut to maxlen bases.  The file is read in PGB200_CHUNK_MB chunks cut at a record
-// boundary, the rest carried into the next chunk.  fgets_piece == 0: pass 1's reader (decode_text: single-line FASTA, 4-line FASTQ),
-// cut at the chunk's last record start, trailing blank lines dropped at the end of the file.  Otherwise the fgets reader (read_text,
-// reader.cu), which reads wrapped records as readseq1by1 / read1seqfq do, in fgets pieces of fgets_piece bytes, and finds the cut.
-void read_file(IMapEngine& eng, const PlanEntry& f, int maxlen, int fgets_piece, std::vector<u64>* words, std::vector<u32>* lens) {
-    std::unique_ptr<FILE, int (*)(FILE*)> file(fopen(f.path.c_str(), "rb"), fclose);
-    if (!file) fail("Cannot open %s. Now exit to system...", f.path.c_str());
-    const size_t cap = (size_t)(getenv("PGB200_CHUNK_MB") ? atoi(getenv("PGB200_CHUNK_MB")) : 256) << 20;
-    std::vector<char> buf(cap + 16);
-    size_t have = 0;
-    bool eof = false;
-    for (;;) {
-        if (!eof) {
-            const size_t got = fread(buf.data() + have, 1, cap - have, file.get());
-            have += got;
-            eof = fgets_piece ? feof(file.get()) != 0 : got == 0;   // pass 1's reader sees the end only in a read that finds nothing
-            if (!eof && ferror(file.get())) fail("pgb200: read error on %s", f.path.c_str());
-        }
-        if (have == 0 && eof) break;
-        size_t cut;
-        try {
-            if (fgets_piece) cut = eng.read_text(buf.data(), have, f.fastq, fgets_piece, maxlen, f.reverse, eof, words, lens);
-            else {
-                if (eof) {
-                    while (have > 1 && buf[have - 1] == '\n' && buf[have - 2] == '\n') have--;
-                    if (have == 1 && buf[0] == '\n') have = 0;
-                }
-                cut = eof ? have : last_record_start(buf.data(), have, f.fastq);
-                eng.decode_text(buf.data(), cut, f.fastq, f.reverse, maxlen, words, lens);
-            }
-        } catch (const std::exception& ex) {
-            if (fgets_piece) fail("%s (%s)", ex.what(), f.path.c_str());
-            fail("readseqInLib return error! please make sure input file is correct fastq/fasta file \n(%s)", ex.what());
-        }
-        if (eof) break;
-        if (cut == 0 && have == cap) fail("pgb200: a single record exceeds the %zu MB chunk", cap >> 20);
-        memmove(buf.data(), buf.data() + cut, have - cut);
-        have -= cut;
+// The stage's reader of read files, with one chunk buffer for the whole stage.  read() appends one file's reads to *words / *lens,
+// each cut to maxlen bases.  fgets_gstr < 0: pass 1's reader (decode_text: single-line FASTA, 4-line FASTQ) with pass 1's record rule.
+// Otherwise the fgets reader (read_text, reader.cu), which reads wrapped records as readseq1by1 / read1seqfq do, in fgets pieces (see
+// load_reads), and finds the cut.
+struct FileReader {
+    IMapEngine& eng;
+    const size_t cap;
+    std::unique_ptr<char[]> buf{new char[cap]};
+    void read(const PlanEntry& f, int maxlen, int fgets_gstr, std::vector<u64>* words, std::vector<u32>* lens) {
+        const int piece = fgets_gstr < 0 ? 0 : fgets_gstr ? f.cut : 4999;
+        read_chunks(f.path, buf.get(), cap, [&](const char* text, size_t n, bool at_eof) {
+            if (piece)
+                return in_step("%s (%s)", [&] { return eng.read_text(text, n, f.fastq, piece, maxlen, f.reverse, at_eof, words, lens); }, f.path.c_str());
+            const size_t cut = whole_records(text, n, f.fastq, at_eof);
+            in_step("readseqInLib return error! please make sure input file is correct fastq/fasta file \n(%s)",
+                    [&] { eng.decode_text(text, cut, f.fastq, f.reverse, maxlen, words, lens); });
+            return cut;
+        });
     }
-}
+};
 
 // One pass's reads, decoded before anything is written: every refusal comes before the first output file.  The stderr lines the
 // reference prints while it reads go to *log, to be printed where the pass prints them.  A read longer than `room` would run past
@@ -224,7 +194,7 @@ void read_file(IMapEngine& eng, const PlanEntry& f, int maxlen, int fgets_piece,
 // cut one base past `room` so that such a read shows.  fgets_gstr < 0: pass 1's reader (single-line FASTA, 4-line FASTQ);
 // otherwise the fgets reader, whose pieces are the cutoff long when the pass allocated gStr (fgets_gstr = 1) and gLineLen - 1 = 4999
 // bytes long when it did not (readseq1by1.c:54-66, prlRead2Ctg.c:826, 1133).
-Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pass, int room, int fgets_gstr, std::string* log) {
+Reads load_reads(FileReader& files, const std::vector<MapLib>& libs, bool long_pass, int room, int fgets_gstr, std::string* log) {
     Reads rd;
     char line[256];
     auto say = [&](const char* fmt, auto... a) { snprintf(line, sizeof line, fmt, a...); *log += line; };
@@ -235,9 +205,6 @@ Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pas
             const PlanEntry& e = L.files[fi];
             const int maxlen = std::min(e.cut, room + 1);
             const size_t before = rd.lens.size();
-            auto read_one = [&](const PlanEntry& pe, std::vector<u64>* w, std::vector<u32>* l) {
-                read_file(eng, pe, maxlen, fgets_gstr < 0 ? 0 : fgets_gstr ? pe.cut : 4999, w, l);
-            };
             if (e.mate == 0) {
                 // openFileInLib names both mates before the first read; mates then alternate r1, r2, r1, r2
                 const PlanEntry& m = L.files[++fi];
@@ -245,8 +212,8 @@ Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pas
                 say("Import reads from file:\n %s\n", m.path.c_str());
                 std::vector<u64> w1, w2;
                 std::vector<u32> l1, l2;
-                read_one(e, &w1, &l1);
-                read_one(m, &w2, &l2);
+                files.read(e, maxlen, fgets_gstr, &w1, &l1);
+                files.read(m, maxlen, fgets_gstr, &w2, &l2);
                 if (l1.size() != l2.size())
                     fail("pgb200: mate files hold different numbers of reads (%zu vs %zu): unsupported", l1.size(), l2.size());
                 const size_t w0 = rd.words.size();
@@ -266,7 +233,7 @@ Reads load_reads(IMapEngine& eng, const std::vector<MapLib>& libs, bool long_pas
                 }
             } else {
                 say("Import reads from file:\n %s\n", e.path.c_str());
-                read_one(e, &rd.words, &rd.lens);
+                files.read(e, maxlen, fgets_gstr, &rd.words, &rd.lens);
             }
             for (size_t r = before; r < rd.lens.size(); r++)
                 if ((int)rd.lens[r] > room)
@@ -379,14 +346,13 @@ struct BatchMapper {
           pl(hit.size()), rc{std::vector<unsigned char>((size_t)read_len, 0)} {}
     const u64* read(u64 t) const { return W + wofs[t]; }
     // returns the host time at which the GPU's placements were in
-    double map(u64 b0, u64 n, int alignlen, bool per_read_cta, const char* what) {
+    double map(u64 b0, u64 n, int alignlen, bool per_read_cta, const char* fail_fmt) {
         const u64 w0 = rd.wofs[b0];
         wofs.resize(n);
         for (u64 t = 0; t < n; t++) wofs[t] = rd.wofs[b0 + t] - w0;
         W = rd.words.data() + w0;
         lens = rd.lens.data() + b0;
-        try { eng.map_batch(W, rd.wofs[b0 + n] - w0, wofs.data(), lens, n, alignlen, per_read_cta, hit.data()); }
-        catch (const std::exception& ex) { fail("pgb200: %s failed: %s", what, ex.what()); }
+        in_step(fail_fmt, [&] { eng.map_batch(W, rd.wofs[b0 + n] - w0, wofs.data(), lens, n, alignlen, per_read_cta, hit.data()); });
         const double t_mapped = host_now();
         rc.chops(n, P, K, lens, W, wofs.data());
         pl.set(hit.data(), n, ci, K, prefix);
@@ -426,7 +392,7 @@ void map_long_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, long 
         const u64 n = std::min<u64>((u64)max_read_num, n_reads - b0);
         last_batch = (long long)n;
         const int alignlen = std::max(plan.long_libs[rd.lib[b0 + n - 1]].map_len, 35);   // ALIGNLEN after the batch's last read (:1198-1204)
-        bm.map(b0, n, alignlen, true, "long-read scan");
+        bm.map(b0, n, alignlen, true, "pgb200: long-read scan failed: %s");
         s_gap.clear(); s_txt.clear();
         for (u64 t = 0; t < n; t++) {   // recordLongRead, output1read (prlRead2Ctg.c:456-492, 612-625)
             read_counter++;
@@ -458,8 +424,7 @@ struct GzOut {
 // prlRead2Ctg once its reads are in: the output files, batches of maxReadNum reads (from max_rd_len), recordAlldgn with its mates
 // (getReadIngap, getPEreadOnContig) and output1read_gz, the closing counts and .peGrads.  long_all: the batches through k_map_long.
 void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, const std::string& log, long long max_read_num, const ContigInfo& ci, int K,
-                     int P, int fill, bool long_all, const std::string& prefix, double* ms_record, double* ms_deflate) {
-    const int device = getenv("PGB200_DEVICE") ? atoi(getenv("PGB200_DEVICE")) : 0;   // map_stage's device
+                     int P, int fill, bool long_all, const std::string& prefix, int device, double* ms_record, double* ms_deflate) {
     GzOut f_gap, f_short, f_on, f_pe;
     f_gap.open(prefix + ".readInGap.gz", device);
     if (fill) f_short.open(prefix + ".shortreadInGap.gz", device);
@@ -482,16 +447,13 @@ void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, cons
     const std::vector<char>&orien = bm.pl.orien, &footprint = bm.pl.footprint;
     long long read_counter = 0, map_counter = 0, in_gap = 0;
     int alignlen = 0, prev_lib = -1;
-    // everything the writer thread touches is declared before its join guard, so it outlives the thread on every way out
-    std::exception_ptr wr_err;
+    // everything the writer thread touches is declared before the writer, whose destructor waits for the thread on every way out
     std::string s_gap, s_short, s_on, s_pe;
-    std::thread writer;
-    struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } join_writer{writer};
+    std::future<void> writer;
     auto join = [&] {
         const double t_join = host_now();
-        if (writer.joinable()) writer.join();
+        if (writer.valid()) writer.get();   // rethrows the writer's failure
         *ms_deflate += host_now() - t_join;
-        if (wr_err) std::rethrow_exception(wr_err);
     };
     long long last_batch = 0;
     for (u64 b0 = 0; b0 < n_reads; b0 += (u64)max_read_num) {
@@ -502,7 +464,7 @@ void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, cons
             if (rd.lib[r] != prev_lib) { prev_lib = rd.lib[r]; alignlen = L.avg_ins > 1000 ? std::max(L.map_len, 35) : std::max(L.map_len, 32); }
             if (L.avg_ins > 1000) alignlen = std::max(alignlen, (int)(rd.lens[r] / 2 + 1));
         }
-        const double t_rec = bm.map(b0, n, alignlen, long_all, "read scan");
+        const double t_rec = bm.map(b0, n, alignlen, long_all, "pgb200: read scan failed: %s");
         // recordAlldgn (prlRead2Ctg.c:627-712) into this batch's byte strings
         join();
         s_gap.clear(); s_short.clear(); s_on.clear(); s_pe.clear();
@@ -548,10 +510,7 @@ void map_short_reads(IMapEngine& eng, const MapPlan& plan, const Reads& rd, cons
         }
         *ms_record += host_now() - t_rec;
         // the deflate runs beside the next batch's GPU work, on the writers' own streams
-        writer = std::thread([&] {
-            try { f_gap.write(s_gap); if (fill) f_short.write(s_short); f_on.write(s_on); if (fill) f_pe.write(s_pe); }
-            catch (...) { wr_err = std::current_exception(); }
-        });
+        writer = std::async(std::launch::async, [&] { f_gap.write(s_gap); if (fill) f_short.write(s_short); f_on.write(s_on); if (fill) f_pe.write(s_pe); });
     }
     join();
     if (n_reads && last_batch != max_read_num) {   // a batch that ends exactly at the last read is recorded inside the reference's loop
@@ -602,9 +561,7 @@ int map_stage(int argc, char** argv, int flavour127) {
     if (K < 13 || K > kmax || K % 2 == 0) fail("pgb200: K %d is outside 13..%d or even", K, kmax);
     if (P < 1) fail("pgb200: -p must be at least 1");
     fprintf(stderr, "Contig length cutoff: %d.\n", K + 2);
-    int device = 0;
-    if (const char* v = getenv("PGB200_DEVICE")) device = atoi(v);
-    const int verbose = getenv("PGB200_VERBOSE") ? atoi(getenv("PGB200_VERBOSE")) : 0;
+    const StageSettings env = stage_settings();
 
     // ---- prlContig2nodes
     double t0 = host_now();
@@ -616,12 +573,10 @@ int map_stage(int argc, char** argv, int flavour127) {
     const MapPlan plan = map_plan(cfg.c_str());
     if (plan.max_rd_len - K + 1 <= 0) fail("pgb200: max_rd_len %d is shorter than K %d", plan.max_rd_len, K);
     const bool long_pass = plan.long_len >= 1;   // prlRead2Ctg.c:1099-1104
-    std::unique_ptr<IMapEngine> eng;
-    try { eng.reset(make_map_engine(K, device)); } catch (const std::exception& ex) { fail("pgb200: %s", ex.what()); }
+    std::unique_ptr<IMapEngine> eng(in_step("pgb200: %s", [&] { return make_map_engine(K, env.device); }));
     const double t_hash = host_now();
     u64 distinct = 0;
-    try { eng->hash_contigs(ctg.packed.data(), ctg.off.back(), ctg.off.data(), ctg.id.data(), ctg.id.size(), &distinct); }
-    catch (const std::exception& ex) { fail("pgb200: contig hash failed: %s", ex.what()); }
+    in_step("pgb200: contig hash failed: %s", [&] { eng->hash_contigs(ctg.packed.data(), ctg.off.back(), ctg.off.data(), ctg.id.data(), ctg.id.size(), &distinct); });
     fprintf(stderr, "Time spent on hashing contigs: %ds.\n", (int)((host_now() - t_hash) * 1e-3));
     fprintf(stderr, "%lli node(s) allocated, %lli kmer(s) in contigs, %lli kmer(s) processed.\n", (long long)distinct, (long long)ctg.n_kmers, (long long)ctg.n_kmers);
     fprintf(stderr, "Time spent on graph construction: %ds.\n\n", (int)((host_now() - t0) * 1e-3));
@@ -634,11 +589,12 @@ int map_stage(int argc, char** argv, int flavour127) {
     // the long pass allocates it for longReadLen > gLineLen (prlRead2Ctg.c:1133), the short pass for max_rd_len > gLineLen (:826).
     const char* reader_env = getenv("PGB200_MAP_READER");
     const bool fgets_short = reader_env && !strcmp(reader_env, "fgets");
-    const Reads lrd = long_pass ? load_reads(*eng, plan.long_libs, true, plan.long_len, plan.long_len > 5000 ? 1 : 0, &long_log) : Reads{};
+    FileReader files{*eng, env.chunk_bytes};
+    const Reads lrd = long_pass ? load_reads(files, plan.long_libs, true, plan.long_len, plan.long_len > 5000 ? 1 : 0, &long_log) : Reads{};
     MapTimes t_lrd;
     eng->times(&t_lrd);
     const double ms_read_long = host_now() - t0;
-    const Reads rd = load_reads(*eng, plan.libs, false, plan.max_rd_len, fgets_short ? (plan.max_rd_len > 5000 ? 1 : 0) : -1, &short_log);
+    const Reads rd = load_reads(files, plan.libs, false, plan.max_rd_len, fgets_short ? (plan.max_rd_len > 5000 ? 1 : 0) : -1, &short_log);
     const double ms_read = host_now() - t0;
     const long long max_read_num = batch_reads("max_rd_len", plan.max_rd_len, K);
     const long long max_long_num = long_pass ? batch_reads("long read length", plan.long_len, K) : 0;
@@ -657,7 +613,7 @@ int map_stage(int argc, char** argv, int flavour127) {
         map_long_reads(*eng, plan, lrd, max_long_num, ci, K, P, fill, prefix);
         print_libs(plan);
         fprintf(stderr, "0 reads deleted.\n");
-        if (verbose) {
+        if (env.verbose) {
             MapTimes tm;
             eng->times(&tm);
             fprintf(stderr, "[pgb200] map long pass: %zu reads, %.0f ms (host), long-read scan %.1f ms (GPU events), %llu lookups; reading %.0f ms (host), "
@@ -676,10 +632,10 @@ int map_stage(int argc, char** argv, int flavour127) {
         fprintf(stderr, "%d edge(s) in the graph.\n", ci.num_all);
     }
     double ms_record = 0, ms_deflate = 0;
-    map_short_reads(*eng, plan, rd, short_log, max_read_num, ci, K, P, fill, long_all, prefix, &ms_record, &ms_deflate);
+    map_short_reads(*eng, plan, rd, short_log, max_read_num, ci, K, P, fill, long_all, prefix, env.device, &ms_record, &ms_deflate);
     print_libs(plan);
     fprintf(stderr, "Time spent on aligning reads: %ds.\n\n", (int)((host_now() - t0) * 1e-3));
-    if (verbose) {
+    if (env.verbose) {
         MapTimes tm;
         eng->times(&tm);
         fprintf(stderr, "[pgb200] map: parse .contig %.0f ms (host), contig hash %.1f ms, read decode %.1f ms, read scan %.1f ms (GPU events); reading %.0f ms, "

@@ -9,9 +9,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <exception>
+#include <future>
 #include <memory>
 #include <stdexcept>
-#include <thread>
 #include <getopt.h>
 #include <cuda_runtime_api.h>
 
@@ -66,10 +66,6 @@ void phase_vertex(IEngine& e, const PgParams& p, const std::string& prefix, pgb2
 }
 
 namespace {
-// Runs f; a failure is rethrown as `fmt` with its message in place of the %s: the text the stage prints for that step.
-template <class F> auto in_step(const char* fmt, F&& f) -> decltype(f()) {
-    try { return f(); } catch (const std::exception& ex) { fail(fmt, ex.what()); }
-}
 // The stage's engines: engine g on GPU device0 + g.  IEngine's methods expect the calling thread to be bound to the engine's GPU
 // (the C-ABI's entry points do that for their callers); at(g) does it here.
 struct Engines {
@@ -102,10 +98,11 @@ struct Engines {
 struct Feeder {
     static constexpr size_t kMaxChunksPerEpoch = 120;   // several GPUs: at most this many chunks (over all GPUs) between collective flushes
     Engines& engs;
+    const size_t cap;         // chunk bytes
     size_t next = 0;          // engine of the next chunk
     char* pin = nullptr;
-    size_t cap = 0, fed_in_epoch = 0;
-    double ms_read = 0, ms_feed = 0;   // wall time inside fread / inside feed_text (PGB200_VERBOSE)
+    size_t fed_in_epoch = 0;
+    double ms_read = 0, ms_feed = 0;   // wall time reading the files, outside the chunks' feed / inside feed_text (PGB200_VERBOSE)
     ~Feeder() { if (pin) cudaFreeHost(pin); }
     void collective_flush() {
         in_step("pgb200: %s", [&] { for (size_t g = 0; g < engs.e.size(); g++) engs.at(g).xchg_fence(); for (size_t g = 0; g < engs.e.size(); g++) engs.at(g).flush(); });
@@ -114,34 +111,14 @@ struct Feeder {
     // streams one file; returns number of records
     uint64_t run(const std::string& fn, bool fastq, uint64_t ord_base, uint64_t ord_stride, int reverse, int maxlen) {
         fprintf(stderr, "Import reads from file:\n %s\n", fn.c_str());
-        std::unique_ptr<FILE, int (*)(FILE*)> file(fopen(fn.c_str(), "rb"), fclose);
-        if (!file) fail("Cannot open %s. Now exit to system...", fn.c_str());
-        if (!pin) {
-            const char* env = getenv("PGB200_CHUNK_MB");
-            cap = (size_t)(env ? atoi(env) : 256) << 20;
-            if (cudaHostAlloc((void**)&pin, cap + 16, cudaHostAllocDefault) != cudaSuccess) { pin = nullptr; fail("pgb200: cudaHostAlloc failed"); }
-        }
+        if (!pin && cudaHostAlloc((void**)&pin, cap + 16, cudaHostAllocDefault) != cudaSuccess) { pin = nullptr; fail("pgb200: cudaHostAlloc failed"); }
         uint64_t recs = 0;
-        size_t have = 0;
-        bool eof = false;
-        while (!eof || have) {
-            const double t_r = host_now();
-            size_t got = eof ? 0 : fread(pin + have, 1, cap - have, file.get());
-            ms_read += host_now() - t_r;
-            if (got == 0) eof = true;
-            have += got;
-            if (have == 0) break;
-            size_t cut;
-            if (eof) {
-                while (have > 1 && pin[have - 1] == '\n' && pin[have - 2] == '\n') have--;   // trailing blank lines are harmless
-                if (have == 1 && pin[0] == '\n') have = 0;
-                if (have == 0) break;
-                cut = have;
-            } else {
-                cut = last_record_start(pin, have, fastq);
-                if (cut == 0 && have == cap) fail("pgb200: a single record exceeds the %zu MB chunk", cap >> 20);
-                if (cut == 0) continue;
-            }
+        const double t_run = host_now();
+        double ms_take = 0;
+        read_chunks(fn, pin, cap, [&](const char* text, size_t n, bool at_eof) {
+            const double t_take = host_now();
+            const size_t cut = whole_records(text, n, fastq, at_eof);
+            if (cut == 0) return cut;
             if (engs.e.size() > 1) {
                 // several GPUs: room for this chunk's records in every arena region, and for its segment (128 per epoch over all GPUs)
                 // reads in this chunk, estimated generously from the library's read length (a record is a header, the bases and,
@@ -153,14 +130,15 @@ struct Feeder {
             const double t_f = host_now();
             IEngine& eng = engs.at(next);
             in_step("readseqInLib return error! please make sure input file is correct fastq/fasta file \n(%s)",
-                    [&] { eng.feed_text(pin, cut, false, fastq, ord_base + recs * ord_stride, ord_stride, reverse, maxlen); });
+                    [&] { eng.feed_text(text, cut, false, fastq, ord_base + recs * ord_stride, ord_stride, reverse, maxlen); });
             ms_feed += host_now() - t_f;
             recs += eng.last_chunk_records();
             next = (next + 1) % engs.e.size();
             fed_in_epoch++;
-            memmove(pin, pin + cut, have - cut);
-            have -= cut;
-        }
+            ms_take += host_now() - t_take;
+            return cut;
+        });
+        ms_read += host_now() - t_run - ms_take;
         return recs;
     }
 };
@@ -219,9 +197,10 @@ int pregraph(int argc, char** argv, int flavour127) {
     if (prm.K % 2 == 0) { prm.K++; fprintf(stderr, "K should be an odd number.\n"); }
     if (prm.K < 13) { prm.K = 13; fprintf(stderr, "K should not be less than 13.\n"); }
     else if (prm.K > (flavour127 ? 127 : 63)) { prm.K = flavour127 ? 127 : 63; fprintf(stderr, "K should not be greater than %d.\n", prm.K); }
-    if (const char* v = getenv("PGB200_DEVICE")) prm.device = atoi(v);
+    const StageSettings env = stage_settings();
+    prm.device = env.device;
+    prm.verbose = env.verbose;
     if (const char* v = getenv("PGB200_TABLE_SLOTS")) prm.table_slots = strtoull(v, nullptr, 10);
-    if (const char* v = getenv("PGB200_VERBOSE")) prm.verbose = atoi(v);
 
     // ---- pass 1 (prlRead2HashTable)
     double t0 = host_now();
@@ -260,7 +239,7 @@ int pregraph(int argc, char** argv, int flavour127) {
         tl.mark("engines");
         uint64_t ord_next = 0, n_reads = 0;
         {
-            Feeder fd{engs};
+            Feeder fd{engs, env.chunk_bytes};
             for (size_t i = 0; i < plan.files.size(); i++) {
                 const PlanEntry& e = plan.files[i];
                 if (e.mate == 0) {
@@ -312,10 +291,8 @@ int pregraph(int argc, char** argv, int flavour127) {
         const std::string edge_text = in_step("pgb200: edges failed: %s", [&] { return phase_edges(engs.at(0), p0, nullptr, nullptr); });
         const uint64_t num_ed = engs.e[0]->num_ed();
         // The deflate of the edge text is sequential host work (it has to be: the bytes must equal the reference's gz stream); it runs
-        // on a host thread while the GPU does pass 2.  The thread is joined on every way out (destroying a joinable one ends the process).
-        std::exception_ptr edge_error;
-        std::thread edge_files([&] { try { write_edge_outputs(prefix, edge_text, p0, num_ed); } catch (...) { edge_error = std::current_exception(); } });
-        struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } join_edge_files{edge_files};
+        // on a host thread while the GPU does pass 2.  get() rethrows its failure; on every other way out the future's destructor waits.
+        std::future<void> edge_files = std::async(std::launch::async, [&] { write_edge_outputs(prefix, edge_text, p0, num_ed); });
         tl.mark("edges");
         fprintf(stderr, "Time spent on constructing edges: %ds.\n\n", seconds_since(t0));
         // ---- pass 2 (prlRead2edge)
@@ -323,9 +300,8 @@ int pregraph(int argc, char** argv, int flavour127) {
         in_step("pgb200: pass 2 failed: %s", [&] { phase_pass2(engs.at(0), p0, prefix, nullptr); });
         fprintf(stderr, "Time spent on aligning reads: %ds.\n\n", seconds_since(t0));
         tl.mark("pass 2 + its files");
-        edge_files.join();
+        edge_files.get();
         tl.mark("waiting for the edge file");
-        if (edge_error) std::rethrow_exception(edge_error);
         in_step("pgb200: vertex output failed: %s", [&] { phase_vertex(engs.at(0), p0, prefix, nullptr); });
     }   // the engine is released here, inside the "vertex + teardown" interval
     tl.mark("vertex + teardown");

@@ -1,14 +1,38 @@
-// stage.h -- what abi.cpp (the C-ABI veneer), stage.cpp (the pregraph stage and its graph phases) and stage_io.cpp (config, chunk
-// cutter, output files, edge sidecar; no GPU) share.  Internal to csrc/: not installed, and hidden from the library's exports.
+// stage.h -- what abi.cpp (the C-ABI veneer), stage.cpp (pregraph and its graph phases), map_stage.cpp (map) and stage_io.cpp (settings,
+// config, chunked reads, output files, edge sidecar; no GPU) share.  Internal to csrc/: not installed, and hidden from the library's exports.
 #pragma once
 #include "../../include/pregraph_b200.h"
 #include "engine.h"
+#include <cstdio>
+#include <exception>
+#include <functional>
 
 #pragma GCC visibility push(hidden)
 namespace pgb {
 
 [[noreturn]] void fail(const char* fmt, ...);     // throws std::runtime_error with the printf-formatted text the stage prints
+// Runs f; a failure is rethrown as `fmt` with its message for the first %s, then a...: the text the stage prints for that step.
+template <class F, class... A> auto in_step(const char* fmt, F&& f, A... a) -> decltype(f()) {
+    try { return f(); } catch (const std::exception& ex) { fail(fmt, ex.what(), a...); }
+}
 PgParams to_pg_params(const pgb200_params& p);   // fills in defaults; checks K range, 16-bit k-mer positions, world / rank
+
+// The environment settings both stages share, read once before any engine exists: PGB200_DEVICE (the stage's first GPU),
+// PGB200_VERBOSE (where the time went) and PGB200_CHUNK_MB (the read files' chunk: a whole number of MB from 1 to 4095, so that a
+// chunk stays under the engines' 4 GiB limit; default 256).
+struct StageSettings { int device = 0, verbose = 0; size_t chunk_bytes = (size_t)256 << 20; };
+StageSettings stage_settings();
+
+FILE* ckopen(const std::string& name, const char* mode);   // fopen, or fail as the reference's ckopen (check.c:30-34)
+std::string read_whole_file(FILE* f);                      // the rest of an open file
+// Reads `path` through buf, cap bytes the caller owns.  take(text, n, at_eof) gets each chunk, which starts at a record start, and
+// returns how many leading bytes it used; the rest starts the next chunk.  at_eof: the text ends at the end of the file (feof after
+// the fread), and take uses all of it.  An empty file makes no call.  A full chunk of which take used nothing fails.
+using ChunkTake = std::function<size_t(const char* text, size_t n, bool at_eof)>;
+void read_chunks(const std::string& path, char* buf, size_t cap, const ChunkTake& take);
+// Pass 1's record rule (single-line FASTA, 4-line FASTQ): the leading bytes of a chunk that hold whole records.  At the end of the
+// file that is all of it but trailing blank lines; otherwise everything before the last record start.
+size_t whole_records(const char* text, size_t n, bool fastq, bool at_eof);
 
 // One implementation per graph phase: each prints the reference's stderr lines and fills its fields of *st (st may be null).
 // phase_edges writes the edge files under `prefix` before its line, or leaves the returned text to the caller (prefix null).

@@ -1,5 +1,5 @@
-// stage_io.cpp -- the stage's host-only work: config, read-stream plan, chunk cutter, output files, edge-sidecar codec.  Mirrors, in
-// new code, the host-side behaviour of (standardPregraph/):
+// stage_io.cpp -- the stages' host-only work: settings, config, read-stream plan, chunked reads, output files, edge-sidecar codec.
+// Mirrors, in new code, the host-side behaviour of (standardPregraph/):
 //   scan_libInfo / splitColumn     lib.c:70-506        (key=value config, [LIB] sections, sort by avg_ins)
 //   openNextFile / nextValidIndex  prlHashReads.c:903-951, readseq1by1.c:595-674 (library + file-type iteration order)
 //   file writers                   prlHashReads.c:1104-1132 (.kmerFreq), node2edge.c:61-70 (.edge.gz via zlib)
@@ -24,6 +24,53 @@ void fail(const char* fmt, ...) {
     throw std::runtime_error(s);
 }
 
+StageSettings stage_settings() {
+    StageSettings s;
+    if (const char* v = getenv("PGB200_DEVICE")) s.device = atoi(v);
+    if (const char* v = getenv("PGB200_VERBOSE")) s.verbose = atoi(v);
+    if (const char* v = getenv("PGB200_CHUNK_MB")) {
+        char* end;
+        const long mb = strtol(v, &end, 10);
+        if (end == v || *end || mb < 1 || mb > 4095) fail("pgb200: PGB200_CHUNK_MB must be a whole number of MB from 1 to 4095, not \"%s\"", v);
+        s.chunk_bytes = (size_t)mb << 20;
+    }
+    return s;
+}
+
+FILE* ckopen(const std::string& name, const char* mode) {
+    FILE* fp = fopen(name.c_str(), mode);
+    if (!fp) fail("Cannot open %s. Now exit to system...", name.c_str());
+    return fp;
+}
+std::string read_whole_file(FILE* f) {
+    std::string s;
+    char buf[1 << 16];
+    size_t got;
+    while ((got = fread(buf, 1, sizeof buf, f)) > 0) s.append(buf, got);
+    return s;
+}
+
+void read_chunks(const std::string& path, char* buf, size_t cap, const ChunkTake& take) {
+    std::unique_ptr<FILE, int (*)(FILE*)> f(ckopen(path, "rb"), fclose);
+    size_t have = 0;
+    for (;;) {
+        have += fread(buf + have, 1, cap - have, f.get());
+        if (ferror(f.get())) fail("pgb200: read error on %s", path.c_str());   // on Linux also a directory, which fopen accepts
+        if (have == 0) return;   // the fread found the end, and nothing was carried
+        const bool at_eof = feof(f.get()) != 0;
+        const size_t used = take(buf, have, at_eof);
+        if (at_eof) return;
+        if (used == 0 && have == cap) fail("pgb200: a single record exceeds the %zu MB chunk", cap >> 20);
+        memmove(buf, buf + used, have - used);
+        have -= used;
+    }
+}
+size_t whole_records(const char* text, size_t n, bool fastq, bool at_eof) {
+    if (!at_eof) return last_record_start(text, n, fastq);
+    while (n > 1 && text[n - 1] == '\n' && text[n - 2] == '\n') n--;   // trailing blank lines are harmless
+    return n == 1 && text[0] == '\n' ? 0 : n;
+}
+
 namespace {   // the library config (lib.c)
 struct Lib {
     int avg_ins = 0, asm_flag = 3, reverse = 0, rd_len_cutoff = 0, map_len = 0, rank = 0, pair_num_cut = 0;
@@ -44,8 +91,7 @@ static bool split_column(const char* line, std::string& a, std::string& b) {   /
     return false;
 }
 static std::vector<Lib> scan_lib(const char* cfg, int* max_rd_len) {
-    FILE* fp = fopen(cfg, "r");
-    if (!fp) fail("Cannot open %s. Now exit to system...", cfg);
+    FILE* fp = ckopen(cfg, "r");
     std::vector<Lib> libs;
     char line[1024];
     std::string a, b;
@@ -167,8 +213,7 @@ size_t last_record_start(const char* buf, size_t n, bool fastq) {
 }
 
 void write_file(const std::string& name, const void* data, size_t n) {
-    FILE* f = fopen(name.c_str(), "wb");
-    if (!f) fail("Cannot open %s. Now exit to system...", name.c_str());   // ckopen, check.c:30-34
+    FILE* f = ckopen(name, "wb");
     if (n && fwrite(data, 1, n, f) != n) { fclose(f); fail("short write on %s", name.c_str()); }
     fclose(f);
 }
@@ -271,10 +316,7 @@ void sidecar_to_edge_gz(const std::string& prefix) {
     const std::string in = prefix + ".edge.b200";
     FILE* f = fopen(in.c_str(), "rb");
     if (!f) fail("pgb200: cannot open %s", in.c_str());
-    std::string raw;
-    char buf[1 << 16];
-    size_t got;
-    while ((got = fread(buf, 1, sizeof buf, f)) > 0) raw.append(buf, got);
+    const std::string raw = read_whole_file(f);
     fclose(f);
     pgb200_edge_sidecar_header h;
     if (raw.size() < sizeof h) fail("pgb200: %s is truncated", in.c_str());
@@ -285,6 +327,7 @@ void sidecar_to_edge_gz(const std::string& prefix) {
     std::string text;
     text.reserve(raw.size() * 4 + (1 << 20));
     size_t off = sizeof h;
+    char buf[512];
     for (uint64_t r = 0; r < h.n_records; r++) {
         int32_t rec[4];
         uint64_t km[8];
@@ -307,6 +350,6 @@ void sidecar_to_edge_gz(const std::string& prefix) {
         if (rec[0] % 100 != 0) text.push_back('\n');
         off += (size_t)rec[3];
     }
-    write_edge_gz(prefix + ".edge.gz", text, getenv("PGB200_DEVICE") ? atoi(getenv("PGB200_DEVICE")) : 0);
+    write_edge_gz(prefix + ".edge.gz", text, stage_settings().device);
 }
 }   // namespace pgb

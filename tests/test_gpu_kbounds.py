@@ -79,8 +79,14 @@ def test_pass1_aggregation_stress_at_word_boundary_k(tmp_path, monkeypatch, _ora
     _pass1_dump(tmp_path, K, True, chunk=700)
 
 
-@pytest.mark.parametrize("K,f127", [(33, False), (33, True), (65, True), (95, True), (97, True)])
-def test_map_at_word_boundary_k(tmp_path, K, f127):
+# chunk_mb: map's default short-pass reader in chunks of that size, which each 1.9 MB read file crosses
+MAP = [(33, False, None), (33, True, None), (65, True, None), (95, True, None), (97, True, None), (33, False, "1")]
+
+
+@pytest.mark.parametrize("K,f127,chunk_mb", MAP, ids=[f"{K}-{f127}" + (f"-chunk{c}mb" if c else "") for K, f127, c in MAP])
+def test_map_at_word_boundary_k(tmp_path, monkeypatch, K, f127, chunk_mb):
+    if chunk_mb:
+        monkeypatch.setenv("PGB200_CHUNK_MB", chunk_mb)
     cfg = synth.scenario_pe_fastq(str(tmp_path))
     g = _graph(str(tmp_path), cfg, K, flavour127=f127)
     _map_both(g, cfg, ["-p", "8"], flavour127=f127)
