@@ -82,7 +82,8 @@ void EngineT<NW>::chop_insert_chunk(const ReadChunk& ch) {
     const unsigned blocks = (unsigned)std::min<u64>((ch.n_rec + INS_THREADS - 1) / INS_THREADS, (u64)n_sm_ * 64);
     const size_t smem = (size_t)INS_THREADS * W64_ * sizeof(u64);
     const int use_tma = smem <= 96 * 1024;
-    if (use_tma && smem > 48 * 1024) cudaFuncSetAttribute(k_chop_insert<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    // opted in for every staged tile: the default limit is 48 KB less the kernel's static shared memory, so a 48 KB tile needs it too
+    if (use_tma) cudaFuncSetAttribute(k_chop_insert<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k_chop_insert<NW><<<blocks, INS_THREADS, use_tma ? smem : 0, st_>>>(tab_, kp_, ch.words, ch.len, ch.n_rec, W64_, ch.ord_base, ch.ord_stride, d_cnt_, use_tma);
     pass_sweeps_ = PassSweeps::Plain;
     PG_CUDA(cudaGetLastError());

@@ -15,6 +15,7 @@
 #include "patch.cuh"
 #include "chop.cuh"
 #include <algorithm>
+#include <cassert>
 
 namespace pgb {
 
@@ -75,6 +76,7 @@ __global__ void __launch_bounds__(128) k_pass2(Table<NW> tab, KParams<NW> kp, co
         const u64* wp = use_tma ? s_words + (u64)threadIdx.x * W64 : words + r * (u64)W64;
         u32* mix = pathbuf + r * (u64)stride;
         const int n = L - K + 1;
+        assert(L <= 32 * W64 && n <= stride - 1);         // the read's words and its path (one entry per k-mer at most) stay in their rows
         Kmer<NW> fwd = kzero<NW>(), rc = kzero<NW>(), prevK = kzero<NW>();
         int retain = 0, pos = 0;
         bool IsPrev = false, stop = false;
@@ -135,6 +137,9 @@ __global__ void __launch_bounds__(128) k_pass2(Table<NW> tab, KParams<NW> kp, co
     if (deleted_reads) atomicAdd(&counters[C_MISC0], (u64)deleted_reads);
 }
 
+// recordPathBin (prlRead2path.c:478-543) counts a path in an unsigned char and stores entry j at fwriteBuf[counter++]: past 255
+// entries the count wraps and later entries overwrite the buffer's start.  It writes the count mod 256 and that many slots, so slot
+// i holds the LAST entry j == i (mod 256) of the path: entry i + 256 * ((cnt - 1 - i) / 256).
 __global__ void __launch_bounds__(128) k_write_paths(const u32* __restrict__ lens, u64 n_rec, int K, u64 ord_base, u64 ord_stride, int stride,
                                                      const u32* pathbuf, const u32* reclen, const u64* recoff, unsigned char* out) {
     for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < n_rec; r += (u64)gridDim.x * blockDim.x) {
@@ -142,10 +147,15 @@ __global__ void __launch_bounds__(128) k_write_paths(const u32* __restrict__ len
         u64 ord = ord_base + r * ord_stride;
         if (!reclen[ord]) continue;
         const u32* mix = pathbuf + r * (u64)stride;
-        u32 cnt = mix[stride - 1] & 255u;
+        const u32 cnt = mix[stride - 1];
+        assert(cnt >= 3 && (int)cnt <= stride - 1);   // k_pass2 records only paths of 3+ entries, at most one per k-mer
+        const u32 c = cnt & 255u;
         unsigned char* o = out + recoff[ord];
-        *o++ = (unsigned char)cnt;
-        for (u32 j = 0; j < cnt; j++) { u32 v = mix[j]; o[0] = v; o[1] = v >> 8; o[2] = v >> 16; o[3] = v >> 24; o += 4; }
+        *o++ = (unsigned char)c;
+        for (u32 j = 0; j < c; j++) {
+            u32 v = mix[j + 256u * ((cnt - 1 - j) >> 8)];
+            o[0] = v; o[1] = v >> 8; o[2] = v >> 16; o[3] = v >> 24; o += 4;
+        }
     }
 }
 
@@ -199,6 +209,8 @@ void EngineT<NW>::pass2(Pass2Stats* st, std::string* prearc_text, std::string* p
         unsigned blocks = (unsigned)std::min<u64>((c.n_rec + 127) / 128, (u64)n_sm_ * 32);
         size_t smem = (size_t)128 * W64_ * sizeof(u64);
         int use_tma = smem <= 48 * 1024;   // longer reads: the unstaged loop
+        // the default limit is 48 KB less the kernel's static shared memory (the mbarrier): opt in so that a 48 KB tile launches
+        if (use_tma) PG_CUDA(cudaFuncSetAttribute(k_pass2<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         k_pass2<NW><<<blocks, 128, use_tma ? smem : 0, st_>>>(tab_, kp_, c.words, c.len, c.n_rec, W64_, c.ord_base, c.ord_stride, stride, pb,
                                              reclenb.template as<u32>(), prm_.repsTie, patch_buf_.template as<PatchSlot<NW>>(), patch_mask_,
                                              quirk128(), arcs, acap - 1, markb.template as<u32>(), d_cnt_, errb.template as<u64>(), use_tma);

@@ -657,3 +657,74 @@ def check_motifs(sets, K: int) -> dict:
         for start, m, end in M.walks:
             assert tip_walk(g, start, K) == (m, _canon(end)[0]), (start, m, end)
     return g
+
+
+# ---------------------------------------------------------------- long read paths for pass 2
+def figure8_long(K: int, revs: list[int], seed: int = 0) -> tuple[_Motifs, list[int]]:
+    """One long read per entry of `revs`, each on its own random sequence and read twice: an entry X of 3K bases ending in G, then a
+    junction k-mer J, then `revs` turns, each a loop a = A..C (4 bases) or b = G...T (5 bases) chosen at random, followed by J again.
+    The loops differ in their first and last base, so J branches on both sides; X's 3K k-mers make a tip too long to clip.  The
+    read's path is revs + 1 edges (the entry edge, then one loop edge per turn), so its .path record holds (revs + 1) & 255 entries:
+    the reference counts a path in an unsigned char.  A path of fewer than 3 edges (revs = 1) gets no record.  Returns (the motif
+    set, the expected record count of each read, None for no record).
+    Reads are 4K + revs * (K + 4.5) bases on average; keep them at or below about 34,000 bases (K = 127: at most 257 turns), the
+    longest the reference was seen to handle (it crashed in pass 1 on reads of 47,707 bases)."""
+    M = _Motifs(K, seed * 1000 + 991 + K)
+    expect = []
+    for n in revs:
+        J = M.seq(K)
+        a = b"A" + M.seq(2) + b"C"
+        b = b"G" + M.seq(3) + b"T"
+        X = M.seq(3 * K - 1) + b"G"
+        turns = [a if t else b for t in M.rng.integers(0, 2, size=n)]
+        if n >= 2:                       # both loops at least once: J has two successors in every read
+            turns[0], turns[1] = a, b
+        M.reads.append((X + J + b"".join(t + J for t in turns), 2))
+        M.walks.append(((X + J)[:K], 3 * K - 1, J))
+        M.expect["nodes"] += 3 * K + 1 + (K + 3 if a in turns else 0) + (K + 4 if b in turns else 0)
+        M.expect["dead_ends"] += 1
+        M.expect["junctions"] += 1
+        expect.append((n + 1) & 255 if n >= 2 else None)
+    return M, expect
+
+
+def write_pass2_scenario(d: str, K: int, revs: list[int], inst: int = 1, seed: int = 0, paired: bool = False, max_rd_len: int = 0,
+                         n_genome: int = 0, rings: int = 0) -> tuple[str, list[int], int]:
+    """`inst` figure8_long reads per entry of `revs` (each read twice), the reads of `rings` branch-free rings (each once), and
+    `n_genome` reads of ragged lengths up to `max_rd_len` from a random genome, shuffled into one FASTA library; or with `paired` only
+    the figure-eight reads, in an f1/f2 pair of files (the two copies of a read are mates).  max_rd_len = 0: the longest read.
+    Returns (config path, the expected .path record count of every figure-eight read that gets a record, in read-stream order, the
+    number of ring reads: pass 2 counts each one as deleted, since no k-mer of a ring lies in an edge)."""
+    M, expect = figure8_long(K, list(revs) * inst, seed)
+    R = _Motifs(K, seed * 1000 + 997 + K)
+    for _ in range(rings):
+        R.ring(2 * K, 3)
+    check_motifs([M, R], K)
+    rng = np.random.default_rng(seed + 31 * K)
+    reads = [(s, e) for (s, _), e in zip(M.reads, expect)]
+    mrl = max_rd_len or max(len(s) for s, _ in reads)
+    assert max(len(s) for s, _ in reads) <= mrl
+    j = lambda n: os.path.join(d, n)
+    if paired:
+        order = rng.permutation(len(reads))
+        write_long(j("p2_1.fa"), [reads[i][0] for i in order], fastq=False, tag="a")
+        write_long(j("p2_2.fa"), [reads[i][0] for i in order], fastq=False, tag="b")
+        files = [("f1", j("p2_1.fa")), ("f2", j("p2_2.fa"))]
+        counts = [reads[i][1] for i in order for _ in range(2)]
+        assert not (n_genome or rings)
+    else:
+        reads = reads * 2
+        if n_genome:
+            g = genome(max(20 * mrl, 40000), seed + 7)
+            lens = rng.integers(K + 1, mrl + 1, size=n_genome)
+            lens[: min(4, n_genome)] = mrl                     # the full row, word for word
+            reads += [(r, None) for r in long_reads_of_lengths(g, [int(x) for x in lens], seed + 8, err=0.002, n_rate=0)]
+        reads += [(r, None) for r, _ in R.reads]
+        order = rng.permutation(len(reads))
+        write_long(j("p2.fa"), [reads[i][0] for i in order], fastq=False, tag="r")
+        files = [("f", j("p2.fa"))]
+        counts = [reads[i][1] for i in order]
+    counts = [c for c in counts if c is not None]
+    cfg = j("p2.cfg")
+    write_config(cfg, mrl, [{"avg_ins": 300 if paired else 200, "files": files}])
+    return cfg, counts, len(R.reads)
