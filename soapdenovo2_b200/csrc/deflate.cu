@@ -16,6 +16,7 @@
 // Streaming: a round runs when the buffer is full.  Not final, it writes every complete block and carries the input from the next
 // block's first byte (and the 32 KB before it), the automaton state there and the partial output byte; the carry is at most one
 // block's input plus the window, so memory is bounded by the buffer whatever the file size.
+#include "cuda_owner.h"
 #include "deflate.cuh"
 #include "deflate.h"
 
@@ -42,8 +43,6 @@ constexpr int CRC_PIECE = 4096;
 constexpr size_t DEFAULT_CHUNK = 32ull << 20;
 constexpr size_t MIN_CHUNK = 5ull << 20;   // > 16383 * 258: every full round completes at least one block
 constexpr size_t CARRY = 8ull << 20;       // >= one block's input + the window + the undecided tail
-
-#define GZ_CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) throw std::runtime_error(std::string("gpu gzip: ") + #x + ": " + cudaGetErrorString(e_)); } while (0)
 
 // ---- hash chains
 __global__ void __launch_bounds__(32) k_hash(const u8* __restrict__ b, i64 nhash, u16* __restrict__ pv) {
@@ -305,36 +304,34 @@ public:
         }
         chunk_ = std::max(chunk ? chunk : DEFAULT_CHUNK, MIN_CHUNK);
         cap_ = chunk_ + CARRY;
-        Dev d(dev_);
-        GZ_CK(cudaStreamCreateWithFlags(&st_, cudaStreamNonBlocking));
-        GZ_CK(cudaMalloc(&buf_[0], cap_ + 64));
-        GZ_CK(cudaMalloc(&buf_[1], cap_ + 64));
-        GZ_CK(cudaMalloc(&G_.changed, sizeof(int)));
-        GZ_CK(cudaMalloc(&crcs_, (cap_ / CRC_PIECE + 2) * sizeof(u32)));
-        GZ_CK(cudaFuncSetAttribute(k_hash, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 * 4));
-        GZ_CK(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, match_smem()));
-        for (u32 i = 0; i < 256; i++) table_[i] = crc_table_entry(i);
+        const pgb::DeviceScope on(dev_);
+        Owners d;   // declared after the scope: released with the device current when a step below throws
+        d.st = pgb::make_stream();
+        for (pgb::DevBuf& b : d.buf) b.alloc(cap_ + 64);
+        d.changed.alloc(sizeof(int));
+        d.crcs.alloc((cap_ / CRC_PIECE + 2) * sizeof(u32));
+        PG_CUDA(cudaFuncSetAttribute(k_hash, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 * 4));
+        PG_CUDA(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, match_smem()));
+        d_ = std::move(d);
+        G_.changed = d_.changed.as<int>();
         x8_piece_ = x8nmodp(CRC_PIECE);
         const u8 hdr[10] = {0x1f, 0x8b, 8, 0, 0, 0, 0, 0, 0, 3};   // no name, no time, xfl 0, OS_CODE 3 (Unix)
         emit(hdr, 10);
     }
     ~GpuGzFile() override {
         try { if (!closed_) close(); } catch (...) {}
-        Dev d(dev_);
-        free_work();
-        for (void* p : {(void*)buf_[0], (void*)buf_[1], (void*)G_.changed, (void*)crcs_}) cudaFree(p);
-        if (st_) cudaStreamDestroy(st_);
+        const pgb::DeviceScope on(dev_);
+        d_ = Owners{};   // the owners leave with this temporary, inside the scope
         if (f_) fclose(f_);
     }
     void write(const void* p, size_t n, bool on_device) override {
         if (closed_) throw std::runtime_error("gpu gzip: write after close");
-        Dev d(dev_);
+        const pgb::DeviceScope on(dev_);
         const u8* q = (const u8*)p;
         while (n) {
             const size_t take = std::min(n, cap_ - (size_t)avail_);
-            if (on_device) GZ_CK(cudaMemcpyAsync(buf_[cur_] + avail_, q, take, cudaMemcpyDeviceToDevice, st_));
-            else GZ_CK(cudaMemcpyAsync(buf_[cur_] + avail_, q, take, cudaMemcpyHostToDevice, st_));
-            GZ_CK(cudaStreamSynchronize(st_));   // the caller may reuse its buffer when write returns
+            PG_CUDA(cudaMemcpyAsync(d_.buf[cur_].as<u8>() + avail_, q, take, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, d_.st));
+            PG_CUDA(cudaStreamSynchronize(d_.st));   // the caller may reuse its buffer when write returns
             avail_ += (i64)take;
             total_ += take;
             q += take;
@@ -345,7 +342,7 @@ public:
     void close() override {
         if (closed_) return;
         closed_ = true;
-        Dev d(dev_);
+        const pgb::DeviceScope on(dev_);
         round(true);
         if (nbits_pend_) { const u8 c = (u8)pend_; emit(&c, 1); }
         u8 tr[8];
@@ -359,43 +356,32 @@ public:
     }
 
 private:
-    struct Dev {   // the writer's device for the duration of a call
-        int old = 0;
-        explicit Dev(int d) { cudaGetDevice(&old); cudaSetDevice(d); }
-        ~Dev() { cudaSetDevice(old); }
-    };
     // The per-position work arrays, sized for a round over n bytes (the first full round sets the size for good; a small file
     // allocates only what it needs).
-    void free_work() {
-        for (void* p : {(void*)pv_, (void*)mt_, (void*)G_.state_at, (void*)G_.symidx_at, (void*)G_.spec, (void*)G_.pre, (void*)syms_,
-                        (void*)segw_, (void*)sege_, (void*)binfo_, (void*)lcode_, (void*)dcode_, (void*)hdr_, (void*)boffs_, (void*)out_})
-            cudaFree(p);
-    }
     void ensure_work(size_t n) {
         n = std::max(n, (size_t)1 << 16);
         if (n <= work_) return;
-        free_work();
-        work_ = n;
-        nseg_max_ = (i64)(n / SEG) + 2;
+        const i64 nseg = (i64)(n / SEG) + 2;
         nblk_max_ = (int)(n / SYM_END) + 3;
-        GZ_CK(cudaMalloc(&pv_, n * sizeof(u16)));
-        GZ_CK(cudaMalloc(&mt_, n * sizeof(u64)));
-        GZ_CK(cudaMalloc(&G_.state_at, (n + 2) * sizeof(u32)));
-        GZ_CK(cudaMalloc(&G_.symidx_at, (n + 2) * sizeof(u16)));
-        GZ_CK(cudaMalloc(&G_.spec, (size_t)nseg_max_ * SEG * sizeof(Sym)));
-        GZ_CK(cudaMalloc(&G_.pre, (size_t)nseg_max_ * SEG * sizeof(Sym)));
-        GZ_CK(cudaMalloc(&syms_, (n + 2) * sizeof(Sym)));
-        GZ_CK(cudaMalloc(&segw_, (size_t)nseg_max_ * 4 * sizeof(u32)));
-        GZ_CK(cudaMalloc(&sege_, (size_t)nseg_max_ * 5 * sizeof(u64)));
-        G_.nspec = segw_; G_.npre = segw_ + nseg_max_; G_.skip = segw_ + 2 * nseg_max_; soffs_ = segw_ + 3 * nseg_max_;
-        G_.spec_exit = sege_; G_.entry = sege_ + nseg_max_; G_.exitA = sege_ + 2 * nseg_max_; G_.exitB = sege_ + 3 * nseg_max_;
-        GZ_CK(cudaMalloc(&binfo_, nblk_max_ * sizeof(BlockOut)));
-        GZ_CK(cudaMalloc(&lcode_, (size_t)nblk_max_ * L_CODES * sizeof(u32)));
-        GZ_CK(cudaMalloc(&dcode_, (size_t)nblk_max_ * D_CODES * sizeof(u32)));
-        GZ_CK(cudaMalloc(&hdr_, (size_t)nblk_max_ * HDR_WORDS * sizeof(u32)));
-        GZ_CK(cudaMalloc(&boffs_, nblk_max_ * sizeof(u64)));
-        out_words_ = (2 * n + (1 << 20)) / 4;
-        GZ_CK(cudaMalloc(&out_, out_words_ * sizeof(u32)));
+        d_.pv.alloc(n * sizeof(u16));
+        d_.mt.alloc(n * sizeof(u64));
+        d_.state_at.alloc((n + 2) * sizeof(u32));
+        d_.symidx_at.alloc((n + 2) * sizeof(u16));
+        d_.spec.alloc((size_t)nseg * SEG * sizeof(Sym));
+        d_.pre.alloc((size_t)nseg * SEG * sizeof(Sym));
+        d_.syms.alloc((n + 2) * sizeof(Sym));
+        d_.segw.alloc((size_t)nseg * 4 * sizeof(u32));
+        d_.sege.alloc((size_t)nseg * 5 * sizeof(u64));
+        d_.binfo.alloc(nblk_max_ * sizeof(BlockOut));
+        d_.lcode.alloc((size_t)nblk_max_ * L_CODES * sizeof(u32));
+        d_.dcode.alloc((size_t)nblk_max_ * D_CODES * sizeof(u32));
+        d_.hdr.alloc((size_t)nblk_max_ * HDR_WORDS * sizeof(u32));
+        d_.boffs.alloc(nblk_max_ * sizeof(u64));
+        d_.out.alloc((2 * n + (1 << 20)) / 4 * sizeof(u32));
+        G_.state_at = d_.state_at.as<u32>(); G_.symidx_at = d_.symidx_at.as<u16>(); G_.spec = d_.spec.as<Sym>(); G_.pre = d_.pre.as<Sym>();
+        G_.nspec = d_.segw.as<u32>(); G_.npre = G_.nspec + nseg; G_.skip = G_.nspec + 2 * nseg; soffs_ = G_.nspec + 3 * nseg;
+        G_.spec_exit = d_.sege.as<u64>(); G_.entry = G_.spec_exit + nseg; G_.exitA = G_.spec_exit + 2 * nseg; G_.exitB = G_.spec_exit + 3 * nseg;
+        work_ = n;   // last: a round after a failed allocation allocates again
     }
     static size_t match_smem() { return (size_t)(MTILE + WSIZE) * 2 + MTILE + WSIZE + MAX_MATCH + 8; }
     void emit(const void* p, size_t n) {
@@ -404,14 +390,14 @@ private:
     }
     void round(bool final) {
         ensure_work((size_t)avail_);
-        Round R{buf_[cur_], buf0_, avail_, final, (i64)(r0_ - buf0_), 0, 0};
+        Round R{d_.buf[cur_].as<u8>(), buf0_, avail_, final, (i64)(r0_ - buf0_), 0, 0};
         // CRC of the bytes this buffer holds for the first time
         if (avail_ > crc_from_) {
             const i64 n = avail_ - crc_from_, np = (n + CRC_PIECE - 1) / CRC_PIECE;
-            k_crc<<<(unsigned)((np + 127) / 128), 128, 0, st_>>>(buf_[cur_] + crc_from_, n, crcs_);
+            k_crc<<<(unsigned)((np + 127) / 128), 128, 0, d_.st>>>(R.b + crc_from_, n, d_.crcs.as<u32>());
             std::vector<u32> c(np);
-            GZ_CK(cudaMemcpyAsync(c.data(), crcs_, np * sizeof(u32), cudaMemcpyDeviceToHost, st_));
-            GZ_CK(cudaStreamSynchronize(st_));
+            PG_CUDA(cudaMemcpyAsync(c.data(), d_.crcs.p, np * sizeof(u32), cudaMemcpyDeviceToHost, d_.st));
+            PG_CUDA(cudaStreamSynchronize(d_.st));
             for (i64 i = 0; i < np; i++) {
                 const u64 len = (u64)std::min((i64)CRC_PIECE, n - i * CRC_PIECE);
                 crc_ = crc_any_ ? multmodp(len == CRC_PIECE ? x8_piece_ : x8nmodp(len), crc_) ^ c[i] : c[i];
@@ -422,52 +408,52 @@ private:
         R.lmatch = final ? avail_ : avail_ - MIN_LOOKAHEAD;
         R.nlt = (final ? avail_ + 1 : R.lmatch) - R.r0;
         const i64 nhash = avail_ - 2;
-        if (nhash > 0) k_hash<<<(unsigned)((nhash + HTILE - 1) / HTILE), 32, 32768 * 4, st_>>>(R.b, nhash, pv_);
+        if (nhash > 0) k_hash<<<(unsigned)((nhash + HTILE - 1) / HTILE), 32, 32768 * 4, d_.st>>>(R.b, nhash, d_.pv.as<u16>());
         if (R.lmatch > R.r0)
-            k_match<<<(unsigned)((R.lmatch - R.r0 + MTILE - 1) / MTILE), MTHREADS, match_smem(), st_>>>(R, pv_, mt_);
+            k_match<<<(unsigned)((R.lmatch - R.r0 + MTILE - 1) / MTILE), MTHREADS, match_smem(), d_.st>>>(R, d_.pv.as<u16>(), d_.mt.as<u64>());
         G_.nseg = (R.nlt + SEG - 1) / SEG;
-        GZ_CK(cudaMemsetAsync(G_.state_at, 0xff, (size_t)R.nlt * sizeof(u32), st_));
+        PG_CUDA(cudaMemsetAsync(G_.state_at, 0xff, (size_t)R.nlt * sizeof(u32), d_.st));
         const unsigned sg = (unsigned)((G_.nseg + 127) / 128);
-        k_lazy_spec<<<sg, 128, 0, st_>>>(R, mt_, G_, pack_state(st0_));
+        k_lazy_spec<<<sg, 128, 0, d_.st>>>(R, d_.mt.as<u64>(), G_, pack_state(st0_));
         for (int pass = 0;; pass++) {
-            GZ_CK(cudaMemsetAsync(G_.changed, 0, sizeof(int), st_));
-            k_lazy_fix<<<sg, 128, 0, st_>>>(R, mt_, G_, G_.exitA, G_.exitB);
+            PG_CUDA(cudaMemsetAsync(G_.changed, 0, sizeof(int), d_.st));
+            k_lazy_fix<<<sg, 128, 0, d_.st>>>(R, d_.mt.as<u64>(), G_, G_.exitA, G_.exitB);
             int ch = 0;
-            GZ_CK(cudaMemcpyAsync(&ch, G_.changed, sizeof(int), cudaMemcpyDeviceToHost, st_));
-            GZ_CK(cudaStreamSynchronize(st_));
+            PG_CUDA(cudaMemcpyAsync(&ch, G_.changed, sizeof(int), cudaMemcpyDeviceToHost, d_.st));
+            PG_CUDA(cudaStreamSynchronize(d_.st));
             std::swap(G_.exitA, G_.exitB);
             if (!ch) break;
         }
         // symbol counts -> offsets
         std::vector<u32> w((size_t)G_.nseg * 3);
-        GZ_CK(cudaMemcpyAsync(w.data(), G_.nspec, G_.nseg * sizeof(u32), cudaMemcpyDeviceToHost, st_));
-        GZ_CK(cudaMemcpyAsync(w.data() + G_.nseg, G_.npre, G_.nseg * sizeof(u32), cudaMemcpyDeviceToHost, st_));
-        GZ_CK(cudaMemcpyAsync(w.data() + 2 * G_.nseg, G_.skip, G_.nseg * sizeof(u32), cudaMemcpyDeviceToHost, st_));
-        GZ_CK(cudaStreamSynchronize(st_));
+        PG_CUDA(cudaMemcpyAsync(w.data(), G_.nspec, G_.nseg * sizeof(u32), cudaMemcpyDeviceToHost, d_.st));
+        PG_CUDA(cudaMemcpyAsync(w.data() + G_.nseg, G_.npre, G_.nseg * sizeof(u32), cudaMemcpyDeviceToHost, d_.st));
+        PG_CUDA(cudaMemcpyAsync(w.data() + 2 * G_.nseg, G_.skip, G_.nseg * sizeof(u32), cudaMemcpyDeviceToHost, d_.st));
+        PG_CUDA(cudaStreamSynchronize(d_.st));
         std::vector<u32> offs(G_.nseg);
         u64 T = 0;
         for (i64 i = 0; i < G_.nseg; i++) { offs[i] = (u32)T; T += w[G_.nseg + i] + w[i] - w[2 * G_.nseg + i]; }
-        GZ_CK(cudaMemcpyAsync(soffs_, offs.data(), G_.nseg * sizeof(u32), cudaMemcpyHostToDevice, st_));
-        k_gather<<<(unsigned)G_.nseg, 256, 0, st_>>>(G_, soffs_, syms_);
+        PG_CUDA(cudaMemcpyAsync(soffs_, offs.data(), G_.nseg * sizeof(u32), cudaMemcpyHostToDevice, d_.st));
+        k_gather<<<(unsigned)G_.nseg, 256, 0, d_.st>>>(G_, soffs_, d_.syms.as<Sym>());
         // blocks: final -- all, an empty last block when an in-loop flush took the last symbol; not final -- the complete ones
         if (!final) {
             if (T < (u64)SYM_END) throw std::runtime_error("gpu gzip: a full buffer holds no complete block");
             T -= T % SYM_END;
         }
         Sym lastsym{0, 0, 0};
-        if (T) GZ_CK(cudaMemcpyAsync(&lastsym, syms_ + T - 1, sizeof(Sym), cudaMemcpyDeviceToHost, st_));
-        GZ_CK(cudaStreamSynchronize(st_));
+        if (T) PG_CUDA(cudaMemcpyAsync(&lastsym, d_.syms.as<Sym>() + T - 1, sizeof(Sym), cudaMemcpyDeviceToHost, d_.st));
+        PG_CUDA(cudaStreamSynchronize(d_.st));
         int nb = (int)(T / SYM_END + (T % SYM_END != 0));
         if (final && T % SYM_END == 0 && !(T && !sym_is_match(lastsym.sym) && (i64)lastsym.pos == avail_ - 1)) nb++;
         if (nb > nblk_max_) throw std::runtime_error("gpu gzip: block table overflow");
-        Blocks K{syms_, T, nb, final, binfo_, lcode_, dcode_, hdr_};
+        Blocks K{d_.syms.as<Sym>(), T, nb, final, d_.binfo.as<BlockOut>(), d_.lcode.as<u32>(), d_.dcode.as<u32>(), d_.hdr.as<u32>()};
         if (nb) {
-            GZ_CK(cudaMemsetAsync(hdr_, 0, (size_t)nb * HDR_WORDS * sizeof(u32), st_));
-            k_block<<<nb, 256, 0, st_>>>(R, K);
+            PG_CUDA(cudaMemsetAsync(d_.hdr.p, 0, (size_t)nb * HDR_WORDS * sizeof(u32), d_.st));
+            k_block<<<nb, 256, 0, d_.st>>>(R, K);
         }
         std::vector<BlockOut> info(nb);
-        if (nb) GZ_CK(cudaMemcpyAsync(info.data(), binfo_, nb * sizeof(BlockOut), cudaMemcpyDeviceToHost, st_));
-        GZ_CK(cudaStreamSynchronize(st_));
+        if (nb) PG_CUDA(cudaMemcpyAsync(info.data(), d_.binfo.p, nb * sizeof(BlockOut), cudaMemcpyDeviceToHost, d_.st));
+        PG_CUDA(cudaStreamSynchronize(d_.st));
         std::vector<u64> boffs(nb);
         u64 bit = (u64)nbits_pend_;
         for (int k = 0; k < nb; k++) {
@@ -476,17 +462,17 @@ private:
         }
         if (final) bit = (bit + 7) & ~7ull;   // bi_windup after the last block
         const size_t words = (size_t)(bit / 32 + 2);
-        if (words > out_words_) throw std::runtime_error("gpu gzip: output buffer overflow");
-        GZ_CK(cudaMemsetAsync(out_, 0, words * sizeof(u32), st_));
-        if (nbits_pend_) GZ_CK(cudaMemcpyAsync(out_, &pend_, sizeof(u32), cudaMemcpyHostToDevice, st_));
+        if (words * sizeof(u32) > d_.out.bytes) throw std::runtime_error("gpu gzip: output buffer overflow");
+        PG_CUDA(cudaMemsetAsync(d_.out.p, 0, words * sizeof(u32), d_.st));
+        if (nbits_pend_) PG_CUDA(cudaMemcpyAsync(d_.out.p, &pend_, sizeof(u32), cudaMemcpyHostToDevice, d_.st));
         if (nb) {
-            GZ_CK(cudaMemcpyAsync(boffs_, boffs.data(), nb * sizeof(u64), cudaMemcpyHostToDevice, st_));
-            k_pack<<<nb, 256, 0, st_>>>(R, K, boffs_, out_);
+            PG_CUDA(cudaMemcpyAsync(d_.boffs.p, boffs.data(), nb * sizeof(u64), cudaMemcpyHostToDevice, d_.st));
+            k_pack<<<nb, 256, 0, d_.st>>>(R, K, d_.boffs.as<u64>(), d_.out.as<u32>());
         }
-        GZ_CK(cudaGetLastError());
+        PG_CUDA(cudaGetLastError());
         std::vector<u8> ob(words * 4);
-        GZ_CK(cudaMemcpyAsync(ob.data(), out_, words * 4, cudaMemcpyDeviceToHost, st_));
-        GZ_CK(cudaStreamSynchronize(st_));
+        PG_CUDA(cudaMemcpyAsync(ob.data(), d_.out.p, words * 4, cudaMemcpyDeviceToHost, d_.st));
+        PG_CUDA(cudaStreamSynchronize(d_.st));
         emit(ob.data(), bit / 8);
         nbits_pend_ = (int)(bit & 7);
         pend_ = nbits_pend_ ? ob[bit / 8] : 0;
@@ -498,8 +484,8 @@ private:
         st0_ = sym_is_match(lastsym.sym) ? fresh_state() : unpack_state(lastsym.next);
         const u64 nb0 = bstart > (u64)WSIZE ? bstart - WSIZE : 0;
         const i64 keep = avail_ - (i64)(nb0 - buf0_);
-        GZ_CK(cudaMemcpyAsync(buf_[cur_ ^ 1], buf_[cur_] + (nb0 - buf0_), keep, cudaMemcpyDeviceToDevice, st_));
-        GZ_CK(cudaStreamSynchronize(st_));
+        PG_CUDA(cudaMemcpyAsync(d_.buf[cur_ ^ 1].p, R.b + (nb0 - buf0_), keep, cudaMemcpyDeviceToDevice, d_.st));
+        PG_CUDA(cudaStreamSynchronize(d_.st));
         cur_ ^= 1;
         crc_from_ -= (i64)(nb0 - buf0_);
         buf0_ = nb0;
@@ -509,26 +495,17 @@ private:
     int dev_;
     std::vector<u8>* mem_;
     FILE* f_ = nullptr;
-    cudaStream_t st_ = nullptr;
     size_t chunk_, cap_, work_ = 0;
-    i64 nseg_max_ = 0;
     int nblk_max_ = 0;
-    u8* buf_[2] = {nullptr, nullptr};
+    // The stream and device memory, released with the writer's device current: ~GpuGzFile resets them inside its DeviceScope.
+    struct Owners {
+        pgb::Stream st;
+        pgb::DevBuf buf[2], changed, crcs;
+        pgb::DevBuf pv, mt, state_at, symidx_at, spec, pre, syms, segw, sege, binfo, lcode, dcode, hdr, boffs, out;   // ensure_work
+    } d_;
     int cur_ = 0;
-    u16* pv_ = nullptr;
-    u64* mt_ = nullptr;
-    Segs G_{};
-    Sym* syms_ = nullptr;
-    u32* segw_ = nullptr;
+    Segs G_{};   // views into d_, as are soffs_ and the kernels' other pointer arguments
     u32* soffs_ = nullptr;
-    u64* sege_ = nullptr;
-    BlockOut* binfo_ = nullptr;
-    u32 *lcode_ = nullptr, *dcode_ = nullptr, *hdr_ = nullptr;
-    u64* boffs_ = nullptr;
-    u32* out_ = nullptr;
-    size_t out_words_ = 0;
-    u32* crcs_ = nullptr;
-    u32 table_[256];
     u32 x8_piece_;
     // stream state
     u64 buf0_ = 0;          // stream offset of the buffer's first byte
@@ -555,7 +532,7 @@ public:
         std::vector<u8> h;
         if (on_device) {
             h.resize(n);
-            GZ_CK(cudaMemcpy(h.data(), p, n, cudaMemcpyDeviceToHost));
+            PG_CUDA(cudaMemcpy(h.data(), p, n, cudaMemcpyDeviceToHost));
             p = h.data();
         }
         size_t off = 0;
@@ -647,12 +624,9 @@ GzFile* gz_open(const std::string& path, int device) {
     if (const char* c = getenv("PGB200_GZ_CHUNK_MB")) chunk = (size_t)atoll(c) << 20;
     // a GPU whose memory the stage has filled cannot hold the writer's buffers (about 60 bytes per byte of a round): zlib writes
     size_t free_b = 0, total_b = 0;
-    int old = 0;
-    cudaGetDevice(&old);
-    cudaSetDevice(device);
+    const pgb::DeviceScope on(device);
     const bool room = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess &&
                       free_b > 64 * (std::max(chunk ? chunk : gz::DEFAULT_CHUNK, gz::MIN_CHUNK) + gz::CARRY) + (256ull << 20);
-    cudaSetDevice(old);
     if (!room) {
         if (verbose()) fprintf(stderr, "[pgb200] gzip: %zu MB free on GPU %d is too little for the writer; %s is written with zlib\n", free_b >> 20, device, path.c_str());
         return gz_open_host(path);

@@ -3,63 +3,17 @@
 // (K <= 127).
 #pragma once
 #include "engine.h"
+#include "cuda_owner.h"
 #include "kmer.cuh"
 #include "table.cuh"
 #include "skm.cuh"
 #include <cuda_runtime.h>
-#include <cstdio>
 #include <cstdlib>
 #include <ctime>
-#include <stdexcept>
 #include <string>
-#include <utility>
 #include <vector>
 
 namespace pgb {
-
-#define PG_CUDA(call)                                                                                         \
-    do {                                                                                                      \
-        cudaError_t e__ = (call);                                                                             \
-        if (e__ != cudaSuccess) {                                                                             \
-            char b__[512];                                                                                    \
-            snprintf(b__, sizeof b__, "CUDA error %s at %s:%d: %s", cudaGetErrorName(e__), __FILE__, __LINE__, \
-                     cudaGetErrorString(e__));                                                                \
-            throw std::runtime_error(b__);                                                                    \
-        }                                                                                                     \
-    } while (0)
-
-struct DevBuf {
-    void* p = nullptr;
-    size_t bytes = 0;
-    DevBuf() {}
-    DevBuf(DevBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
-    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(bytes, o.bytes); return *this; }
-    ~DevBuf() { release(); }
-    void alloc(size_t n) {
-        release();
-        if (n == 0) n = 16;
-        PG_CUDA(cudaMalloc(&p, n));
-        bytes = n;
-    }
-    void ensure(size_t n) { if (n > bytes) alloc(n + n / 4); }
-    void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
-    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-// Owner of a stream, an event or a pinned host block, in the style of DevBuf: released with its owner, moved but never copied.
-template <class T, cudaError_t (*Release)(T)>
-struct CudaOwned {
-    T h = nullptr;
-    CudaOwned() {}
-    CudaOwned(CudaOwned&& o) noexcept : h(o.h) { o.h = nullptr; }
-    CudaOwned& operator=(CudaOwned&& o) noexcept { std::swap(h, o.h); return *this; }
-    ~CudaOwned() { if (h) Release(h); }
-    operator T() const { return h; }
-};
-template <class T> cudaError_t free_pinned(T* p) { return cudaFreeHost(p); }
-using Stream = CudaOwned<cudaStream_t, cudaStreamDestroy>;
-using Event = CudaOwned<cudaEvent_t, cudaEventDestroy>;
-template <class T> using Pinned = CudaOwned<T*, free_pinned<T>>;
 
 inline u64 next_pow2(u64 x) { u64 p = 1; while (p < x) p <<= 1; return p; }
 
@@ -212,7 +166,8 @@ public:
     // the exchange arena: [SKM_ARENA_HALVES][nseg | ring | offsets | world x cap_pair records]; xa_peer_[o] = owner o's arena as mapped here
     SkmArenaGeom xa_geom_;
     DevBuf xa_buf_;
-    std::vector<void*> xa_peer_, xa_ipc_opened_;
+    std::vector<void*> xa_peer_;
+    std::vector<IpcMapping> xa_ipc_opened_;
     u64 xa_send_epoch_ = 0, xa_flushed_epoch_ = 0;
     u32 xa_seg_idx_ = 0;
     std::vector<u64> xa_reads_cum_;   // reads fed in this epoch after 0, 1, 2, ... chunks (the fill known to the host lags behind)

@@ -255,9 +255,9 @@ public:
         kp_ = make_kparams<NW>(K);
         PG_CUDA(cudaSetDevice(device));
         PG_CUDA(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device));
-        PG_CUDA(cudaStreamCreateWithFlags(&st_.h, cudaStreamNonBlocking));
-        PG_CUDA(cudaEventCreate(&ev_[0].h)); PG_CUDA(cudaEventCreate(&ev_[1].h));
-        PG_CUDA(cudaHostAlloc(&h_cnt_.h, (C_COUNT + 2) * sizeof(u64), cudaHostAllocDefault));
+        st_ = make_stream();
+        for (Event& e : ev_) e = make_event();
+        h_cnt_ = make_pinned<u64>(C_COUNT + 2);
         cnt_.alloc(C_COUNT * sizeof(u64));
         PG_CUDA(cudaMemsetAsync(cnt_.p, 0, C_COUNT * sizeof(u64), st_));
     }

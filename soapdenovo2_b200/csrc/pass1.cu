@@ -454,27 +454,25 @@ EngineT<NW>::EngineT(const PgParams& p) : prm_(p) {
     }
     if (p.world > 1) skm_mode_ = 1;   // records are the only exchange format
     kp_ = make_kparams<NW>(p.K);
-    for (Stream* s : {&st_, &st_copy_, &st_clear_, &st_dec_}) PG_CUDA(cudaStreamCreateWithFlags(&s->h, cudaStreamNonBlocking));
-    for (Event* e : {&ev_clear_, &ev_dec_done_, &ev_copy_}) PG_CUDA(cudaEventCreateWithFlags(&e->h, cudaEventDisableTiming));
-    PG_CUDA(cudaEventCreate(&ev_flush_begin_.h));
-    PG_CUDA(cudaEventCreate(&ev_flush_.h));
-    for (auto& q : ev_ring_) for (Event& e : q) PG_CUDA(cudaEventCreate(&e.h));
-    PG_CUDA(cudaHostAlloc(&h_outcome_.h, sizeof(FlushOutcome), cudaHostAllocDefault));
+    for (Stream* s : {&st_, &st_copy_, &st_clear_, &st_dec_}) *s = make_stream();
+    for (Event* e : {&ev_clear_, &ev_dec_done_, &ev_copy_}) *e = make_event(cudaEventDisableTiming);
+    for (Event* e : {&ev_flush_begin_, &ev_flush_}) *e = make_event();
+    for (auto& q : ev_ring_) for (Event& e : q) e = make_event();
+    h_outcome_ = make_pinned<FlushOutcome>(1);
     cnt_buf_.alloc(C_COUNT * sizeof(u64));
     d_cnt_ = cnt_buf_.template as<u64>();
     PG_CUDA(cudaMemsetAsync(d_cnt_, 0, C_COUNT * sizeof(u64), st_));
-    PG_CUDA(cudaHostAlloc(&h_cnt_.h, (C_COUNT + 2) * sizeof(u64), cudaHostAllocDefault));
+    h_cnt_ = make_pinned<u64>(C_COUNT + 2);
     for (int i = 0; i < C_COUNT; i++) h_cnt_[i] = 0;
     W64_ = (p.max_rd_len + 31) / 32;
     if (W64_ < 1) W64_ = 1;
     sync();
 }
 
-// The members release their memory, streams and events; nothing of this engine may still be running by then.
+// The members release their memory, streams, events and IPC mappings after this body; nothing of this engine may still be running by then.
 template <int NW>
 EngineT<NW>::~EngineT() {
     for (cudaStream_t s : {st_.h, st_dec_.h, st_copy_.h, st_clear_.h}) cudaStreamSynchronize(s);
-    for (void* p : xa_ipc_opened_) cudaIpcCloseMemHandle(p);
 }
 
 template class EngineT<2>;

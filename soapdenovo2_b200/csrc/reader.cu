@@ -411,8 +411,6 @@ __global__ void k_fg_tail(const unsigned char* __restrict__ text, u64 nbytes, co
 }
 
 // ---------------------------------------------------------------------------------------------- host
-FgetsReader::FgetsReader() { PG_CUDA(cudaHostAlloc(&h_.h, FG_SLOTS * sizeof(u64) + 16, cudaHostAllocDefault)); }
-
 size_t FgetsReader::read(const unsigned char* d_text, size_t nbytes, int fastq, int piece_len, int cutoff, int reverse, bool at_eof, int n_sm,
                          cudaStream_t st, std::vector<u64>* words, std::vector<u32>* lens) {
     if (nbytes == 0) return 0;
@@ -421,6 +419,7 @@ size_t FgetsReader::read(const unsigned char* d_text, size_t nbytes, int fastq, 
     const u64 P = (u64)piece_len;
     slots_.ensure(FG_SLOTS * sizeof(u64));
     u64* slots = slots_.as<u64>();
+    if (!h_) h_ = make_pinned<u64>(FG_SLOTS + 2);   // made on first use, with the caller's device current
     u64* h = h_.h;
     PG_CUDA(cudaMemsetAsync(slots, 0, FG_SLOTS * sizeof(u64), st));
     scan_.ensure(scan_scratch_elems(nbytes + 2) * sizeof(u64) + 256);

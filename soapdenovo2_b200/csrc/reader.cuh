@@ -15,7 +15,6 @@ constexpr int FG_NAME_MAX = 256;   // the reference's read_name holds maxNameLen
 // Throws on a NUL byte and on a header name longer than FG_NAME_MAX, before anything is appended.
 class FgetsReader {
 public:
-    FgetsReader();
     size_t read(const unsigned char* d_text, size_t nbytes, int fastq, int piece_len, int cutoff, int reverse, bool at_eof, int n_sm, cudaStream_t st,
                 std::vector<u64>* words, std::vector<u32>* lens);
 

@@ -282,7 +282,7 @@ void EngineT<NW>::xchg_import(int peer, const void* handle64) {
     void* p = nullptr;
     PG_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
     xa_peer_[peer] = p;
-    xa_ipc_opened_.push_back(p);
+    xa_ipc_opened_.emplace_back(p);
 }
 template <int NW>
 void EngineT<NW>::xchg_import_ptr(int peer, int peer_device, void* base) {

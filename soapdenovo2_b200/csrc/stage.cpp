@@ -13,7 +13,7 @@
 #include <memory>
 #include <stdexcept>
 #include <getopt.h>
-#include <cuda_runtime_api.h>
+#include "cuda_owner.h"
 
 namespace pgb {
 void phase_tips(IEngine& e, const PgParams& p, pgb200_graph_stats* st) {
@@ -100,10 +100,9 @@ struct Feeder {
     Engines& engs;
     const size_t cap;         // chunk bytes
     size_t next = 0;          // engine of the next chunk
-    char* pin = nullptr;
+    Pinned<char> pin;
     size_t fed_in_epoch = 0;
     double ms_read = 0, ms_feed = 0;   // wall time reading the files, outside the chunks' feed / inside feed_text (PGB200_VERBOSE)
-    ~Feeder() { if (pin) cudaFreeHost(pin); }
     void collective_flush() {
         in_step("pgb200: %s", [&] { for (size_t g = 0; g < engs.e.size(); g++) engs.at(g).xchg_fence(); for (size_t g = 0; g < engs.e.size(); g++) engs.at(g).flush(); });
         fed_in_epoch = 0;
@@ -111,7 +110,7 @@ struct Feeder {
     // streams one file; returns number of records
     uint64_t run(const std::string& fn, bool fastq, uint64_t ord_base, uint64_t ord_stride, int reverse, int maxlen) {
         fprintf(stderr, "Import reads from file:\n %s\n", fn.c_str());
-        if (!pin && cudaHostAlloc((void**)&pin, cap + 16, cudaHostAllocDefault) != cudaSuccess) { pin = nullptr; fail("pgb200: cudaHostAlloc failed"); }
+        if (!pin) in_step("pgb200: cudaHostAlloc failed", [&] { pin = make_pinned<char>(cap + 16); });
         uint64_t recs = 0;
         const double t_run = host_now();
         double ms_take = 0;
