@@ -1,11 +1,11 @@
 // map_stage.cpp -- the `map -s cfg -g prefix [-f] [-p n] [-k k] [-h len]` stage (call_align).  Mirrors, in new code, the host-side
 // behaviour of (standardPregraph/):
 //   call_align / initenv / getMinOverlap   map.c:48-240           (getopt string, K from .preGraphBasic, -k, stderr lines)
-//   prlContig2nodes (host part)            prlHashCtg.c:325-467   (.contig parsing, which contigs are kept, their ids)
+//   prlContig2nodes (host part)            prlHashCtg.c:325-467   (the stats lines; .contig itself is read by read_contigs, stage_io.cpp)
 //   basicContigInfo                        prlRead2Ctg.c:727-763  (.ContigIndex -> lengths, bal_edge)
 //   prlRead2Ctg / recordAlldgn / getReadIngap / output1read_gz / getPEreadOnContig   prlRead2Ctg.c:427-712, 779-1053
 //   prlLongRead2Ctg / recordLongRead / output1read         prlRead2Ctg.c:456-492, 612-625, 1080-1298
-// The k-mer work (contig table, read scan, parse1read) runs on the GPU (map.cu); the .contig text is parsed here, on the host: it is a
+// The k-mer work (contig table, read scan, parse1read) runs on the GPU (map.cu); the .contig text is parsed on the host: it is a
 // few hundred MB at most, multi-line, and is read once.
 //
 // Long-read libraries (asm_flags=4) are mapped first, when getMaxLongReadLen >= 1, and write .longReadInGap (.RlongReadInGap with
@@ -57,80 +57,6 @@ int min_overlap(const std::string& prefix) {   // getMinOverlap, map.c:48-76
         if (line[0] == 'V') sscanf(line + 6, "%d %c %d", &n, &ch, &K);
     fclose(fp);
     return K;
-}
-
-// The kept contigs of <prefix>.contig, their bases packed 2 bits each into one stream (LSB first)
-struct Contigs {
-    std::vector<u64> packed, off{0};
-    std::vector<u32> id;
-    u64 n_kmers = 0;
-};
-Contigs read_contigs(const std::string& prefix, int K) {
-    FILE* fp = ckopen(prefix + ".contig", "r");
-    const std::string text = read_whole_file(fp);
-    fclose(fp);
-    // readseqpar (readseq1by1.c:225-277): record count and the length / name extremes, from the line lengths
-    long long num = -1;
-    int max_len = 10, min_len = 1000, name_len = 10, n = 0;
-    size_t p = 0;
-    std::vector<std::pair<size_t, size_t>> lines;
-    while (p < text.size()) {
-        size_t e = text.find('\n', p);
-        const size_t end = e == std::string::npos ? text.size() : e + 1;
-        lines.push_back({p, end});
-        p = end;
-    }
-    for (auto& L : lines) {
-        if (text[L.first] == '>') {
-            if (num >= 0) { max_len = std::max(max_len, n); min_len = std::min(min_len, n); }
-            n = 0;
-            num++;
-            char nm[5000] = "";
-            sscanf(text.c_str() + L.first + 1, "%4999s", nm);
-            name_len = std::max(name_len, (int)strlen(nm));
-        } else n += (int)(L.second - L.first) - 1;
-    }
-    max_len = std::max(max_len, n); min_len = std::min(min_len, n);
-    num++;
-    fprintf(stderr, "\n%lld contig(s), maximum sequence length %d, minimum sequence length %d, maximum name length %d.\n", num, max_len, min_len, name_len);
-    // readseq1by1 per record: '#' lines skipped, letters -> base codes, '.' -> A, other bytes dropped
-    Contigs c;
-    std::vector<u8> codes;
-    u64 n_bases = 0, ordinal = 0;
-    auto close_record = [&](u32 cid) {
-        ordinal++;
-        const int len = (int)codes.size();
-        if (len >= K + 1 && len >= K + 2) {   // prlHashCtg.c:405 with len_cut = ctg_short = K + 2
-            c.id.push_back(cid > 0 ? cid : (u32)ordinal);
-            for (u8 b : codes) {
-                if ((n_bases & 31) == 0) c.packed.push_back(0);
-                c.packed.back() |= (u64)b << (2 * (n_bases & 31));
-                n_bases++;
-            }
-            c.off.push_back(n_bases);
-            c.n_kmers += (u64)(len - K + 1);
-        }
-        codes.clear();
-    };
-    bool open = false;
-    u32 cid = 0;
-    for (auto& L : lines) {
-        const char* s = text.c_str() + L.first;
-        if (s[0] == '#') continue;
-        if (s[0] == '>') {
-            if (open) close_record(cid);
-            open = true;
-            cid = (s[1] >= '0' && s[1] <= '9') ? (u32)atoi(s + 1) : 0u;   // getID, prlHashCtg.c:297-307
-            continue;
-        }
-        for (size_t i = 0; i < L.second - L.first; i++) {
-            const unsigned ch = (unsigned char)s[i];
-            if ((ch >= 'a' && ch <= 'z') || (ch >= 'A' && ch <= 'Z')) codes.push_back((u8)((ch & 6u) >> 1));
-            else if (ch == '.') codes.push_back(0);
-        }
-    }
-    if (open) close_record(cid);
-    return c;
 }
 
 // basicContigInfo: contig_array[1..num_all].{length, bal_edge}

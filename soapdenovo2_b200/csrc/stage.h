@@ -33,6 +33,15 @@ void read_chunks(const std::string& path, char* buf, size_t cap, const ChunkTake
 // Pass 1's record rule (single-line FASTA, 4-line FASTQ): the leading bytes of a chunk that hold whole records.  At the end of the
 // file that is all of it but trailing blank lines; otherwise everything before the last record start.
 size_t whole_records(const char* text, size_t n, bool fastq, bool at_eof);
+// The contigs of <prefix>.contig that map hashes, read as prlContig2nodes reads them: readseqpar's pass over fgets pieces of 4949 bytes
+// (its stats line goes to stderr), then readseq1by1's pieces of 4999 bytes, each record cut at readseqpar's maximum length, kept if
+// it has at least K + 2 bases.  Bases are packed 2 bits each into one stream (LSB first); record r is [off[r], off[r + 1]).
+struct Contigs {
+    std::vector<unsigned long long> packed, off{0};
+    std::vector<unsigned> id;   // atoi of a name that starts with a digit, else the record's ordinal (1-based, every record counted)
+    unsigned long long n_kmers = 0;
+};
+Contigs read_contigs(const std::string& prefix, int K);
 
 // One implementation per graph phase: each prints the reference's stderr lines and fills its fields of *st (st may be null).
 // phase_edges writes the edge files under `prefix` before its line, or leaves the returned text to the caller (prefix null).

@@ -3,9 +3,11 @@
 //   scan_libInfo / splitColumn     lib.c:70-506        (key=value config, [LIB] sections, sort by avg_ins)
 //   openNextFile / nextValidIndex  prlHashReads.c:903-951, readseq1by1.c:595-674 (library + file-type iteration order)
 //   file writers                   prlHashReads.c:1104-1132 (.kmerFreq), node2edge.c:61-70 (.edge.gz via zlib)
+//   map's .contig reader           prlHashCtg.c:297-425, readseq1by1.c:50-136, 225-277 (getID, prlContig2nodes, readseq1by1, readseqpar)
 #include "stage.h"
 #include "deflate.h"
 #include <algorithm>
+#include <cctype>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -69,6 +71,93 @@ size_t whole_records(const char* text, size_t n, bool fastq, bool at_eof) {
     if (!at_eof) return last_record_start(text, n, fastq);
     while (n > 1 && text[n - 1] == '\n' && text[n - 2] == '\n') n--;   // trailing blank lines are harmless
     return n == 1 && text[0] == '\n' ? 0 : n;
+}
+
+namespace {
+// fgets(str, size, fp) over a file's text: each piece is at most size - 1 bytes and ends after the first '\n'.  eof is feof after
+// the call: a piece that ran into the end of the text before its '\n' or its size limit sets it, as does a call at the end.
+struct Fgets {
+    const std::string& t;
+    size_t at = 0;
+    bool eof = false;
+    bool next(size_t size, const char** s, size_t* n) {
+        if (at == t.size()) { eof = true; return false; }
+        const size_t lim = std::min(t.size(), at + size - 1);
+        const char* nl = (const char*)memchr(t.data() + at, '\n', lim - at);
+        const size_t end = nl ? (size_t)(nl - t.data()) + 1 : lim;
+        eof = !nl && end - at < size - 1;
+        *s = t.data() + at;
+        *n = strnlen(*s, end - at);   // strlen(str): the piece up to a NUL byte
+        at = end;
+        return true;
+    }
+};
+// sscanf(&str[1], "%s", name) on a '>' piece: leading whitespace skipped; a piece with no token leaves name as it was
+void scan_name(const char* s, size_t n, std::string* name) {
+    size_t i = 1;
+    while (i < n && isspace((unsigned char)s[i])) i++;
+    size_t j = i;
+    while (j < n && !isspace((unsigned char)s[j])) j++;
+    if (j > i) name->assign(s + i, j - i);
+}
+}   // namespace
+
+Contigs read_contigs(const std::string& prefix, int K) {
+    FILE* fp = ckopen(prefix + ".contig", "r");
+    const std::string text = read_whole_file(fp);
+    fclose(fp);
+    const char* s;
+    size_t n;
+    std::string name;
+    // readseqpar (readseq1by1.c:225-277): pieces of fgets(str, 4950); each piece but a '>' one adds strlen - 1 to the record's length
+    long long num = -1;
+    int max_len = 10, min_len = 1000, name_len = 10, len = 0;
+    for (Fgets f{text}; f.next(4950, &s, &n);) {
+        if (s[0] != '>') { len += (int)n - 1; continue; }
+        if (num >= 0) { max_len = std::max(max_len, len); min_len = std::min(min_len, len); }
+        len = 0;
+        num++;
+        scan_name(s, n, &name);
+        name_len = std::max(name_len, (int)name.size());
+    }
+    max_len = std::max(max_len, len); min_len = std::min(min_len, len);
+    fprintf(stderr, "\n%lld contig(s), maximum sequence length %d, minimum sequence length %d, maximum name length %d.\n", num + 1, max_len, min_len, name_len);
+    // prlContig2nodes' loop (prlHashCtg.c:393-425) over readseq1by1 (readseq1by1.c:50-136) with gStr NULL: pieces of
+    // fgets(str, gLineLen = 5000), '#' pieces skipped, each record cut where strlen + bases > maxReadLen = max_len
+    Fgets f{text};
+    std::vector<unsigned char> codes;
+    auto record = [&] {   // one record's bases, up to the next '>' piece (whose name is the next record's) or the end
+        codes.clear();
+        while (f.next(5000, &s, &n)) {
+            if (s[0] == '#') continue;
+            if (s[0] == '>') { scan_name(s, n, &name); return; }
+            const size_t room = (size_t)max_len - codes.size(), m = std::min(n, room);
+            for (size_t i = 0; i < m; i++) {
+                const unsigned ch = (unsigned char)s[i];
+                if ((ch >= 'a' && ch <= 'z') || (ch >= 'A' && ch <= 'Z')) codes.push_back((unsigned char)((ch & 6u) >> 1));   // base2int
+                else if (ch == '.') codes.push_back(0);
+            }
+        }
+    };
+    Contigs c;
+    name.clear();   // next_name starts empty (ckalloc is calloc)
+    record();       // the bytes before the first '>' are read and dropped
+    unsigned long long n_bases = 0;
+    for (unsigned ordinal = 1; !f.eof; ordinal++) {
+        const unsigned cid = name[0] >= '0' && name[0] <= '9' ? (unsigned)atoi(name.c_str()) : 0u;   // getID, prlHashCtg.c:297-307
+        record();
+        const int clen = (int)codes.size();
+        if (clen < K + 1 || clen < K + 2) continue;   // len_cut = ctg_short = K + 2
+        c.id.push_back(cid > 0 ? cid : ordinal);
+        for (unsigned char b : codes) {
+            if ((n_bases & 31) == 0) c.packed.push_back(0);
+            c.packed.back() |= (unsigned long long)b << (2 * (n_bases & 31));
+            n_bases++;
+        }
+        c.off.push_back(n_bases);
+        c.n_kmers += (unsigned long long)(clen - K + 1);
+    }
+    return c;
 }
 
 namespace {   // the library config (lib.c)
