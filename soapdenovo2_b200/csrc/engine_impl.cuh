@@ -144,6 +144,8 @@ public:
     // layout
     u64 n_nodes_ = 0;           // distinct k-mers == entries in iteration order
     DevBuf order_buf_;          // u64 order[n_nodes_] : iteration index -> ktab slot
+    // growth replay (no -a): per set, 1 if the set ends at its growth threshold and a later instance makes the reference grow it
+    std::vector<uint32_t> late_growth(const std::vector<u64>& cnt, const std::vector<u64>& first, const u64* sort_keys);
 
     // edges / pass 2 state
     u64 num_ed_ = 0;

@@ -11,9 +11,11 @@
 // every distinct k-mer walks from its home slot doing atomicMin(slot, rank); whoever holds the larger rank moves on
 // (carrying the displaced rank if it won).  The fixed point is exactly the sequential layout.  Ranks are unique
 // (read ordinal << 16 | position), so the 64-bit slot word needs no payload; a second pass lets every k-mer find its
-// own rank again, a third turns the rank table into "position -> ktab slot", and one scan compacts it into order[].
+// own rank again (one lap of its set at most: a key that misses its rank is an error, not a hang), a third turns the rank table
+// into "position -> ktab slot", and one scan compacts it into order[].  Without -a the sets' growth history is replayed instead (f1).
 #include "engine_impl.cuh"
 #include "scan.cuh"
+#include "chop.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <algorithm>
 #include <thread>
@@ -78,17 +80,21 @@ __global__ void __launch_bounds__(256) k_layout_place(Table<NW> tab, RefGeom g, 
     }
 }
 
+// A key whose rank is nowhere in its set (a placement bug) gives up after one lap and counts itself in `lost`
 template <int NW>
-__global__ void __launch_bounds__(256) k_layout_resolve(Table<NW> tab, RefGeom g, const u64* R, u64* gpos_out) {
+__global__ void __launch_bounds__(256) k_layout_resolve(Table<NW> tab, RefGeom g, const u64* R, u64* gpos_out, u64* lost) {
     u64 n = tab.mask + 1;
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         const Slot<NW>* s = tab.slots + i;
         if (!slot_occupied(s)) { continue; }
         const RefPlace p = ref_place(g, slot_key(s));
         const u64* base = R + p.base;
-        u64 pos = p.home;
+        u64 pos = p.home, steps = 0;
         u64 r = s->aux;
-        while (base[pos] != r) { if (++pos == p.size) pos = 0; }
+        while (base[pos] != r) {
+            if (++steps == p.size) { atomicAdd((unsigned long long*)lost, 1ull); break; }
+            if (++pos == p.size) pos = 0;
+        }
         gpos_out[i] = p.base + pos;
     }
 }
@@ -125,7 +131,8 @@ struct OrderOut {
 // depends on the whole growth history.  The history is a function of the keys' first-occurrence order alone (growth k happens
 // when the set holds exactly its first max_k distinct keys), so it can be replayed after the fact: the GPU sorts the distinct
 // k-mers by (set, rank) (library radix sort: plumbing outside the metric) and each set is replayed by one host thread with
-// the same put / grow rules.  Cost O(distinct); only runs when -a is absent.
+// the same put / grow rules.  Cost O(distinct); only runs when -a is absent.  The one growth the keys' order does not fix is that of
+// a set ending exactly at its threshold: the check before a later HIT grows it.  late_growth decides those sets from the read store.
 template <int NW>
 __global__ void __launch_bounds__(256) k_replay_keys(Table<NW> tab, RefGeom g, u64* sort_key, u64* sort_val, u64* cursor) {
     u64 n = tab.mask + 1;
@@ -149,11 +156,60 @@ __global__ void __launch_bounds__(256) k_fill_R(const u64* slots_sorted, const u
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) R[gpos[i]] = slots_sorted[i];
 }
 
-// one reference set, replayed on the host: keys[0..n) in first-occurrence order; returns the final size and pos[i]
+// The growth check fires before every put_kmerset, hits included.  A set whose final count equals its threshold therefore grows once
+// more iff some pass-1 instance of the set comes after its last new key L in the read stream, i.e. has a larger rank than L's first
+// occurrence.  The first check below says which sets end so; k_late_instances decides the rest from the read store.
+constexpr float REF_LOAD = 0.77f;
+// encap_kmerset's new size for a set of `size` slots holding `count` keys (newhash.c:368-375)
+static u64 ref_grown_size(u64 size, u64 count) {
+    u64 nn = size;
+    do { if (nn < 0xFFFFFFFULL) nn <<= 1; else nn += 0xFFFFFFULL; nn = ref_next_prime(nn); } while (nn * REF_LOAD < count + 1);
+    return nn;
+}
+// whether a dynamic set that took n distinct keys holds exactly its growth threshold (793 of 1031, 1588 of 2063, ...) at the end
+static bool ref_ends_at_threshold(u64 n) {
+    u64 size = ref_next_prime(1024), mx = (u64)(size * REF_LOAD);
+    while (n > mx) { size = ref_grown_size(size, mx); mx = (u64)(size * REF_LOAD); }   // growth when the count stands at mx
+    return n && n == mx;
+}
+
+// Sets that end at their threshold: late[s] = the rank of the set's last new key (EMPTY64 for the other sets); grow[s] = 1 once an
+// instance of set s with a larger rank is found.  One thread per read from `r0` on; only instances ranked above `r_min` (the smallest
+// late[]) are hashed.
+struct LateArgs {
+    const u64* late;
+    u32* grow;
+    int P;
+    u64 r_min;
+};
 template <int NW>
-static u64 replay_one_set(const u64* keys, u64 n, bool flavour127, std::vector<u32>& slot /* out: index+1 per slot */) {
+struct LateSink {
+    LateArgs a;
+    u64 rank_base;
+    __device__ __forceinline__ void operator()(const Kmer<NW>& canon, unsigned, unsigned, int j) {
+        const u64 r = rank_base | (u64)j;
+        if (r <= a.r_min) return;
+        const u64 s = crc_hash(canon) % (u64)a.P;
+        if (r > a.late[s] && !a.grow[s]) a.grow[s] = 1;
+    }
+};
+template <int NW>
+__global__ void __launch_bounds__(256) k_late_instances(KParams<NW> kp, const u64* __restrict__ words, const u32* __restrict__ lens, u64 r0,
+                                                        u64 n_rec, int W64, u64 ord_base, u64 ord_stride, LateArgs a) {
+    for (u64 r = r0 + (u64)blockIdx.x * blockDim.x + threadIdx.x; r < n_rec; r += (u64)gridDim.x * blockDim.x) {
+        const int L = (int)lens[r];
+        if (L < kp.K + 1) continue;   // the reference drops these reads before chopping them
+        LateSink<NW> sink{a, (ord_base + r * ord_stride) << 16};
+        chop_read(kp, words + r * (u64)W64, L, sink);
+    }
+}
+
+// one reference set, replayed on the host: keys[0..n) in first-occurrence order; returns the final size and pos[i].  grow_at_end: the
+// set ends at its threshold and a later instance of it makes the reference grow it once more.
+template <int NW>
+static u64 replay_one_set(const u64* keys, u64 n, bool flavour127, bool grow_at_end, std::vector<u32>& slot /* out: index+1 per slot */) {
     u64 size = ref_next_prime(1024);
-    const float lf = 0.77f;
+    const float lf = REF_LOAD;
     u64 mx = (u64)(size * lf), count = 0;
     slot.assign(size, 0);
     auto home = [&](u64 idx, u64 sz) {
@@ -163,8 +219,7 @@ static u64 replay_one_set(const u64* keys, u64 n, bool flavour127, std::vector<u
     };
     std::vector<unsigned char> oldocc, newocc;
     auto grow = [&]() {   // encap_kmerset, dynamic branch (newhash.c:368-452)
-        u64 nn = size;
-        do { if (nn < 0xFFFFFFFULL) nn <<= 1; else nn += 0xFFFFFFULL; nn = ref_next_prime(nn); } while (nn * lf < count + 1);
+        u64 nn = ref_grown_size(size, count);
         u64 old = size;
         oldocc.assign(old, 0);
         for (u64 j = 0; j < old; j++) oldocc[j] = slot[j] != 0;
@@ -193,10 +248,50 @@ static u64 replay_one_set(const u64* keys, u64 n, bool flavour127, std::vector<u
         slot[hc] = (u32)(i + 1);
         count++;
     }
-    // the check also fires on hits: a set that ends exactly at its threshold grows at its next (repeat) instance, which
-    // exists unless the set's last new k-mer is also its very last instance in the read stream (not tracked; assumed)
-    if (n && count + 1 > mx) grow();
+    if (grow_at_end) grow();   // the check on a later hit (decided by k_late_instances)
     return size;
+}
+
+// Which sets grow once more after their last new key: cnt[s] = distinct keys of set s, first[s] = where its keys start in sort_keys
+// (the (set << 56 | rank) keys sorted on the device).  Scans the read store only when some set ends at its threshold.
+template <int NW>
+std::vector<u32> EngineT<NW>::late_growth(const std::vector<u64>& cnt, const std::vector<u64>& first, const u64* sort_keys) {
+    const int P = prm_.P;
+    std::vector<u64> late(P, EMPTY64);
+    std::vector<u32> grow(P, 0);
+    int n_late = 0;
+    for (int i = 0; i < P; i++) {
+        if (!ref_ends_at_threshold(cnt[i])) continue;
+        PG_CUDA(cudaMemcpyAsync(&late[i], sort_keys + first[i + 1] - 1, sizeof(u64), cudaMemcpyDeviceToHost, st_));
+        n_late++;
+    }
+    u64 scanned = 0;
+    if (n_late) {
+        sync();
+        u64 r_min = EMPTY64;
+        for (int i = 0; i < P; i++)
+            if (late[i] != EMPTY64) { late[i] &= (1ull << 56) - 1; r_min = std::min(r_min, late[i]); }
+        DevBuf b;
+        b.alloc(P * (sizeof(u64) + sizeof(u32)));
+        const LateArgs a{b.template as<u64>(), reinterpret_cast<u32*>(b.template as<u64>() + P), P, r_min};
+        PG_CUDA(cudaMemcpyAsync(const_cast<u64*>(a.late), late.data(), P * sizeof(u64), cudaMemcpyHostToDevice, st_));
+        PG_CUDA(cudaMemsetAsync(a.grow, 0, P * sizeof(u32), st_));
+        const u64 ord_min = r_min >> 16;   // the read of the earliest such key
+        for (const ReadChunk& c : chunks_) {
+            const u64 r0 = c.ord_base >= ord_min ? 0 : (ord_min - c.ord_base + c.ord_stride - 1) / c.ord_stride;
+            if (r0 >= c.n_rec) continue;
+            scanned += c.n_rec - r0;
+            const unsigned blocks = (unsigned)std::min<u64>((c.n_rec - r0 + 255) / 256, (u64)n_sm_ * 8);
+            k_late_instances<NW><<<blocks, 256, 0, st_>>>(kp_, c.words, c.len, r0, c.n_rec, W64_, c.ord_base, c.ord_stride, a);
+            PG_CUDA(cudaGetLastError());
+        }
+        PG_CUDA(cudaMemcpyAsync(grow.data(), a.grow, P * sizeof(u32), cudaMemcpyDeviceToHost, st_));
+        sync();
+    }
+    if (prm_.verbose)
+        fprintf(stderr, "[pgb200] layout: %d set(s) end at a growth threshold, %d grow at a later instance, %llu read(s) scanned\n", n_late,
+                (int)std::count(grow.begin(), grow.end(), 1u), (unsigned long long)scanned);
+    return grow;
 }
 
 template <int NW>
@@ -257,12 +352,13 @@ void EngineT<NW>::build_layout() {
         sync();
         std::vector<u64> first(P + 1, 0);
         for (int i = 0; i < P; i++) first[i + 1] = first[i] + cnt[i];
+        const std::vector<u32> grow_at_end = late_growth(cnt, first, kb2.template as<u64>());
         std::vector<std::vector<u32>> slots(P);
         {
             std::vector<std::thread> th;
             const bool f127 = prm_.flavour127 != 0;
             for (int i = 0; i < P; i++)
-                th.emplace_back([&, i]() { set_size[i] = replay_one_set<NW>(h_keys.data() + first[i] * NW, cnt[i], f127, slots[i]); });
+                th.emplace_back([&, i]() { set_size[i] = replay_one_set<NW>(h_keys.data() + first[i] * NW, cnt[i], f127, grow_at_end[i] != 0, slots[i]); });
             for (auto& t : th) t.join();
         }
         u64 total = 0;
@@ -295,8 +391,13 @@ void EngineT<NW>::build_layout() {
     PG_CUDA(cudaMemsetAsync(Rb.p, 0xFF, total * sizeof(u64), st_));
     u64* R = Rb.template as<u64>();
     RefGeom g{d_size, d_base, P, prm_.flavour127 != 0};
+    PG_CUDA(cudaMemsetAsync(d_cnt_ + C_MISC1, 0, sizeof(u64), st_));
     k_layout_place<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, g, R);
-    k_layout_resolve<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, g, R, gposb.template as<u64>());
+    k_layout_resolve<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, g, R, gposb.template as<u64>(), d_cnt_ + C_MISC1);
+    PG_CUDA(cudaGetLastError());
+    read_counters();
+    if (h_cnt_[C_MISC1])
+        throw std::runtime_error("pgb200: internal error: " + std::to_string(h_cnt_[C_MISC1]) + " k-mer(s) did not find their rank in the reference layout");
     k_layout_fill<NW><<<n_sm_ * 8, 256, 0, st_>>>(tab_, gposb.template as<u64>(), R);
     PG_CUDA(cudaGetLastError());
     order_from(R, total);
